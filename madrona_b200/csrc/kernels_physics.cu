@@ -549,6 +549,21 @@ __device__ __forceinline__ bool rotationIsNormalizeFixpoint(Quat q)
 
 constexpr u32 kUnknownSlot = 0x7fffu;
 
+// Slot of a body inside its world's body list: archetypes ascending, rows in
+// order (-1: not a body archetype).  Contacts carry it (Candidate::slots) and the
+// solvers stage bodies by it, so both must use this one formula.
+__device__ __forceinline__ i32 worldBodySlot(const EngineState &S, const PhysicsState &P, const i32 w,
+                                             const u32 arch, const i32 row)
+{
+    i32 slot_base = 0;
+    for (u32 bi = 0; bi < P.numBodyArchetypes; bi++) {
+        const TableDesc &bt = S.tables[P.bodies[bi].archetype];
+        if (P.bodies[bi].archetype == arch) return slot_base + (row - bt.worldOffsets[w]);
+        slot_base += bt.worldCounts[w];
+    }
+    return -1;
+}
+
 // ---- candidate pairs: one warp per world, CPU iteration order -----------------------------
 
 struct PairVisitor {
@@ -640,18 +655,8 @@ __device__ void phaseFindCandidates(EngineState &S, const PhysicsState &P, const
         }
         return;
     }
-    // slot of a body inside its world's body list: archetypes ascending, rows in order
     auto bodySlotInfo = [&](u32 arch, i32 row, bool is_static) -> u32 {
-        i32 slot_base = 0;
-        i32 slot = -1;
-        for (u32 bi = 0; bi < P.numBodyArchetypes; bi++) {
-            const TableDesc &bt = S.tables[P.bodies[bi].archetype];
-            if (P.bodies[bi].archetype == arch) {
-                slot = slot_base + (row - bt.worldOffsets[w]);
-                break;
-            }
-            slot_base += bt.worldCounts[w];
-        }
+        const i32 slot = worldBodySlot(S, P, w, arch, row);
         bool is_mutable = true;
         if (is_static) is_mutable = !rotationIsNormalizeFixpoint(locCol<Quat>(S, P, arch, row, PCRotation));
         const u32 s15 = (slot < 0 || slot >= (i32)kUnknownSlot) ? kUnknownSlot : (u32)slot;
@@ -2021,46 +2026,120 @@ __device__ __forceinline__ void localArms(const PPosRot &pre1, const PPosRot &pr
     *r2 = pre2.q.inv().rotateVec(p2 - pre2.x);
 }
 
-__device__ __forceinline__ BodyPair bodyPair(const EngineState &S, const PhysicsState &P,
-                                             const PObjectManager &objs, u32 a1, i32 r1, u32 a2, i32 r2,
-                                             float *mu_s, float *mu_d)
+// What the solves need of a body's object metadata, with its response type
+// applied: a static body has no inverse mass or inertia.
+struct BodyMass {
+    float invM;
+    Vector3 invI;
+    float muS, muD;
+};
+
+__device__ __forceinline__ BodyMass loadBodyMass(const EngineState &S, const PhysicsState &P,
+                                                 const PObjectManager &objs, u32 arch, i32 row)
 {
-    const PMetadata m1 = objs.metadata[locCol<i32>(S, P, a1, r1, PCObjectID)];
-    const PMetadata m2 = objs.metadata[locCol<i32>(S, P, a2, r2, PCObjectID)];
-    BodyPair bp { m1.invMass, m2.invMass, m1.invInertia, m2.invInertia };
-    if (locCol<u32>(S, P, a1, r1, PCResponseType) == kRespStatic) {
-        bp.invM1 = 0.f;
-        bp.invI1 = Vector3::zero();
+    const PMetadata m = objs.metadata[locCol<i32>(S, P, arch, row, PCObjectID)];
+    BodyMass bm { m.invMass, m.invInertia, m.muS, m.muD };
+    if (locCol<u32>(S, P, arch, row, PCResponseType) == kRespStatic) {
+        bm.invM = 0.f;
+        bm.invI = Vector3::zero();
     }
-    if (locCol<u32>(S, P, a2, r2, PCResponseType) == kRespStatic) {
-        bp.invM2 = 0.f;
-        bp.invI2 = Vector3::zero();
-    }
+    return bm;
+}
+
+__device__ __forceinline__ BodyPair bodyPair(const BodyMass &m1, const BodyMass &m2, float *mu_s, float *mu_d)
+{
     *mu_s = 0.5f * (m1.muS + m2.muS);
     *mu_d = 0.5f * (m1.muD + m2.muD);
-    return bp;
+    return BodyPair { m1.invM, m2.invM, m1.invI, m2.invI };
+}
+
+// ---- per-world body staging of the position solve ---------------------------------------------
+// The position sweep and the joints read and rewrite the same few dozen bodies
+// level after level.  The lanes that own a world first copy each body's x, q and
+// BodyMass into shared memory; contacts and joints work on those copies, and the
+// epilogue writes x, q back.  A body is staged when its world slot (worldBodySlot,
+// also carried by Contact::refInfo / altInfo) is below kStagedBodies; the others,
+// including bodies of unknown slot, are read and written in the global columns
+// through the same accessors.  Staged or not depends on the slot alone, so every
+// body has exactly one live copy during the solve and results do not depend on
+// kStagedBodies.  Slots count rows awaiting compaction too: room (33 bodies) fits,
+// arena's highest slots spill.  A block of 64 threads stages 32 * kPhysWarps /
+// kSolverLanes worlds: 13.6 KB of static shared memory at 16 lanes per world.
+constexpr int kStagedBodies = 48;
+
+struct PosBody {                // x, q read / write
+    Vector3 x;
+    Quat q;
+    BodyMass m;
+};
+
+__device__ __forceinline__ bool isStaged(u32 info) { return (info >> 1) < (u32)kStagedBodies; }
+
+__device__ __forceinline__ PosBody globalPosBody(const EngineState &S, const PhysicsState &P,
+                                                 const PObjectManager &objs, u32 arch, i32 row)
+{
+    return PosBody { locCol<Vector3>(S, P, arch, row, PCPosition), locCol<Quat>(S, P, arch, row, PCRotation),
+                     loadBodyMass(S, P, objs, arch, row) };
+}
+
+// info: (slot << 1) | mutable, as in Contact::refInfo
+__device__ __forceinline__ PosBody loadPosBody(const EngineState &S, const PhysicsState &P,
+                                               const PObjectManager &objs, const PosBody *stage,
+                                               u32 info, u32 arch, i32 row)
+{
+    return isStaged(info) ? stage[info >> 1] : globalPosBody(S, P, objs, arch, row);
+}
+
+__device__ __forceinline__ void storePosBody(const EngineState &S, const PhysicsState &P, PosBody *stage,
+                                             u32 info, u32 arch, i32 row, Vector3 x, Quat q)
+{
+    if (isStaged(info)) {
+        stage[info >> 1].x = x;
+        stage[info >> 1].q = q;
+    } else {
+        locCol<Vector3>(S, P, arch, row, PCPosition) = x;
+        locCol<Quat>(S, P, arch, row, PCRotation) = q;
+    }
+}
+
+// fn(slot, arch, row) for every live body of world w with a staged slot, spread
+// over the LPW lanes (sub = lane in group) that own w
+template <int LPW, typename Fn>
+__device__ __forceinline__ void forEachStagedBody(const EngineState &S, const PhysicsState &P, const i32 w,
+                                                  const int sub, Fn &&fn)
+{
+    for (u32 bi = 0; bi < P.numBodyArchetypes; bi++) {
+        const u32 arch = P.bodies[bi].archetype;
+        const TableDesc &t = S.tables[arch];
+        const i32 first = t.worldOffsets[w];
+        const i32 end = first + t.worldCounts[w];
+        const i32 *world_col = (const i32 *)t.columns[1];
+        for (i32 row = first + sub; row < end; row += LPW) {
+            if (world_col[row] != w) continue;   // destroyed, awaiting compaction
+            const i32 slot = worldBodySlot(S, P, w, arch, row);
+            if ((u32)slot < (u32)kStagedBodies) fn(slot, arch, row);
+        }
+    }
 }
 
 // normal push-out along the contact normal + static friction (xpbd.cpp:347-419, 454-550)
 __device__ void solveContactPosition(EngineState &S, const PhysicsState &P, const PObjectManager &objs,
-                                     Contact &c)
+                                     PosBody *stage, Contact &c)
 {
     c.lambdaN = 0.f;
 
-    Vector3 &x1_ref = locCol<Vector3>(S, P, c.refArch, c.refRow, PCPosition);
-    Vector3 &x2_ref = locCol<Vector3>(S, P, c.altArch, c.altRow, PCPosition);
-    Quat &q1_ref = locCol<Quat>(S, P, c.refArch, c.refRow, PCRotation);
-    Quat &q2_ref = locCol<Quat>(S, P, c.altArch, c.altRow, PCRotation);
+    const PosBody b1 = loadPosBody(S, P, objs, stage, c.refInfo, c.refArch, c.refRow);
+    const PosBody b2 = loadPosBody(S, P, objs, stage, c.altInfo, c.altArch, c.altRow);
     const PPosRot prev1 = locCol<PPosRot>(S, P, c.refArch, c.refRow, PCPrevState);
     const PPosRot prev2 = locCol<PPosRot>(S, P, c.altArch, c.altRow, PCPrevState);
     const PPosRot pre1 = locCol<PPosRot>(S, P, c.refArch, c.refRow, PCPreSolvePos);
     const PPosRot pre2 = locCol<PPosRot>(S, P, c.altArch, c.altRow, PCPreSolvePos);
 
     float mu_s, mu_d;
-    const BodyPair bp = bodyPair(S, P, objs, c.refArch, c.refRow, c.altArch, c.altRow, &mu_s, &mu_d);
+    const BodyPair bp = bodyPair(b1.m, b2.m, &mu_s, &mu_d);
 
-    Vector3 x1 = x1_ref, x2 = x2_ref;
-    Quat q1 = q1_ref, q2 = q2_ref;
+    Vector3 x1 = b1.x, x2 = b2.x;
+    Quat q1 = b1.q, q2 = b2.q;
 
     Vector3 mean;
     float deepest;
@@ -2099,10 +2178,8 @@ __device__ void solveContactPosition(EngineState &S, const PhysicsState &P, cons
         }
     }
 
-    x1_ref = x1;
-    x2_ref = x2;
-    q1_ref = q1;
-    q2_ref = q2;
+    storePosBody(S, P, stage, c.refInfo, c.refArch, c.refRow, x1, q1);
+    storePosBody(S, P, stage, c.altInfo, c.altArch, c.altRow, x2, q2);
 }
 
 __device__ void angularCorrection(Quat &q1, Quat &q2, const BodyPair &bp, Vector3 axis_world, float theta)
@@ -2123,7 +2200,7 @@ __device__ void angularCorrection(Quat &q1, Quat &q2, const BodyPair &bp, Vector
 
 // fixed / hinge joints (xpbd.cpp:552-718)
 __device__ void solveJoint(EngineState &S, const PhysicsState &P, const PObjectManager &objs,
-                           const PJoint &j)
+                           PosBody *stage, const i32 w, const PJoint &j)
 {
     if (j.e1ID < 0 || j.e2ID < 0 || j.e1ID >= S.entityCapacity || j.e2ID >= S.entityCapacity) return;
     const EntitySlot s1 = S.entitySlots[j.e1ID];
@@ -2132,16 +2209,17 @@ __device__ void solveJoint(EngineState &S, const PhysicsState &P, const PObjectM
     const u32 a1 = (u32)s1.a, a2 = (u32)s2.a;
     const i32 r1row = s1.b, r2row = s2.b;
     if (!isBodyArchetype(a1) || !isBodyArchetype(a2)) return;
+    // slot info as in Contact::refInfo (the mutable bit is not read here)
+    const u32 info1 = (u32)worldBodySlot(S, P, w, a1, r1row) << 1;
+    const u32 info2 = (u32)worldBodySlot(S, P, w, a2, r2row) << 1;
 
-    Vector3 &x1_ref = locCol<Vector3>(S, P, a1, r1row, PCPosition);
-    Vector3 &x2_ref = locCol<Vector3>(S, P, a2, r2row, PCPosition);
-    Quat &q1_ref = locCol<Quat>(S, P, a1, r1row, PCRotation);
-    Quat &q2_ref = locCol<Quat>(S, P, a2, r2row, PCRotation);
-    Vector3 x1 = x1_ref, x2 = x2_ref;
-    Quat q1 = q1_ref, q2 = q2_ref;
+    const PosBody b1 = loadPosBody(S, P, objs, stage, info1, a1, r1row);
+    const PosBody b2 = loadPosBody(S, P, objs, stage, info2, a2, r2row);
+    Vector3 x1 = b1.x, x2 = b2.x;
+    Quat q1 = b1.q, q2 = b2.q;
 
     float mu_s, mu_d;
-    const BodyPair bp = bodyPair(S, P, objs, a1, r1row, a2, r2row, &mu_s, &mu_d);
+    const BodyPair bp = bodyPair(b1.m, b2.m, &mu_s, &mu_d);
 
     Vector3 correction;
     if (j.type == 0) {
@@ -2184,10 +2262,8 @@ __device__ void solveJoint(EngineState &S, const PhysicsState &P, const PObjectM
         correction /= cmag;
         positionalCorrection(x1, x2, q1, q2, j.r1, j.r2, bp, correction, cmag, 0);
     }
-    x1_ref = x1;
-    x2_ref = x2;
-    q1_ref = q1;
-    q2_ref = q2;
+    storePosBody(S, P, stage, info1, a1, r1row, x1, q1);
+    storePosBody(S, P, stage, info2, a2, r2row, x2, q2);
 }
 
 // Contact sweep of one world by a group of LPW lanes (32 / LPW worlds share a
@@ -2198,10 +2274,14 @@ __device__ void solveJoint(EngineState &S, const PhysicsState &P, const PObjectM
 // levels inside a chunk run in order, so any two contacts sharing a mutable body
 // keep their sequential order.  Inside a level the members are compacted onto
 // the group's first lanes (ballot + find-nth-set).
-// The solves are latency bound with ~4 contacts per level, so several worlds per
-// warp multiply the worlds in flight per SM at no register cost.
+// Several worlds per warp multiply the worlds in flight per SM at no register
+// cost.  Measured on room at 8192 worlds (H100, staged position solve): 16 lanes
+// per world 1.515 ms/step (position solve 0.371, velocity solve 0.256 ms/step),
+// 8 lanes 1.537 (0.426, 0.225), parent code at 8 lanes 1.604 (0.496, 0.219).
+// 4 lanes does not fit: 16 staged worlds per block exceed 48 KB of static
+// shared memory.
 #ifndef MB2_SOLVER_LPW
-#define MB2_SOLVER_LPW 8
+#define MB2_SOLVER_LPW 16
 #endif
 constexpr int kSolverLanes = MB2_SOLVER_LPW;
 
@@ -2246,30 +2326,45 @@ __device__ __forceinline__ void sweepContactLevels(const Contact *contacts, cons
     }
 }
 
-// Joints follow the contacts, sequentially.
+// Joints follow the contacts, sequentially.  stage: [kStagedBodies] of world w.
 __device__ void phaseSolvePositions(EngineState &S, const PhysicsState &P, const i32 w, const bool valid,
-                                    const int lane)
+                                    const int lane, PosBody *stage)
 {
     const PObjectManager &objs = worldObjects(S, P, w);
+    const int sub = lane & (kSolverLanes - 1);
+    if (valid) {
+        forEachStagedBody<kSolverLanes>(S, P, w, sub, [&](i32 slot, u32 arch, i32 row) {
+            stage[slot] = globalPosBody(S, P, objs, arch, row);
+        });
+    }
+    __syncwarp();
 
     Contact *contacts = P.contacts + (size_t)w * P.maxCandidatesPerWorld;
     const i32 *order = P.contactOrder + (size_t)w * P.maxContactsPerWorld;
     const i32 n = valid ? P.contactCounts[w] : 0;
     const i32 levels = valid ? P.contactMaxLevel[w] : 0;
     sweepContactLevels<kSolverLanes>(contacts, order, n, levels, lane, [&](i32 i) {
-        solveContactPosition(S, P, objs, contacts[i]);
+        solveContactPosition(S, P, objs, stage, contacts[i]);
     });
 
     const TableDesc &jt = S.tables[P.jointArchetype];
-    if (valid && (lane & (kSolverLanes - 1)) == 0 && jt.numRows > 0) {
+    if (valid && sub == 0 && jt.numRows > 0) {
         const PJoint *joints = (const PJoint *)jt.columns[P.jointCol];
         const i32 *jw = (const i32 *)jt.columns[1];
         const i32 first = jt.worldOffsets[w];
         const i32 count = jt.worldCounts[w];
         for (i32 r = first; r < first + count; r++) {
             if (jw[r] < 0) continue;
-            solveJoint(S, P, objs, joints[r]);
+            solveJoint(S, P, objs, stage, w, joints[r]);
         }
+    }
+    __syncwarp();
+
+    if (valid) {
+        forEachStagedBody<kSolverLanes>(S, P, w, sub, [&](i32 slot, u32 arch, i32 row) {
+            locCol<Vector3>(S, P, arch, row, PCPosition) = stage[slot].x;
+            locCol<Quat>(S, P, arch, row, PCRotation) = stage[slot].q;
+        });
     }
 }
 
@@ -2294,7 +2389,8 @@ __device__ void solveContactVelocity(EngineState &S, const PhysicsState &P, cons
     const PVelocity pv2 = locCol<PVelocity>(S, P, c.altArch, c.altRow, PCPreSolveVel);
 
     float mu_s, mu_d;
-    const BodyPair bp = bodyPair(S, P, objs, c.refArch, c.refRow, c.altArch, c.altRow, &mu_s, &mu_d);
+    const BodyPair bp = bodyPair(loadBodyMass(S, P, objs, c.refArch, c.refRow),
+                                 loadBodyMass(S, P, objs, c.altArch, c.altRow), &mu_s, &mu_d);
 
     Vector3 v1 = vel1_ref.linear, o1 = vel1_ref.angular;
     Vector3 v2 = vel2_ref.linear, o2 = vel2_ref.angular;
@@ -2374,6 +2470,8 @@ __device__ void solveContactVelocity(EngineState &S, const PhysicsState &P, cons
     vel2_ref = PVelocity { v2, o2 };
 }
 
+// Not staged: with the velocity sweep's shorter load chains, copying every body
+// in and out cost more than the sweep saved (DESIGN.md 3.2).
 __device__ void phaseSolveVelocities(EngineState &S, const PhysicsState &P, const i32 w, const bool valid,
                                      const int lane)
 {
@@ -2390,8 +2488,10 @@ __device__ void phaseSolveVelocities(EngineState &S, const PhysicsState &P, cons
 
 // =============================================================================================
 // Launchers.  Row-parallel phases (leaf update, refit, integrate, velocity
-// update) are grid-stride kernels over all rows of every body archetype;
-// per-world phases (candidates, narrowphase, solves) give each world a warp.
+// update) are grid-stride kernels over all rows of every body archetype; the
+// candidate search gives each world a warp, the solves give each world
+// kSolverLanes lanes (and the position solve a shared-memory copy of its
+// bodies, kStagedBodies).
 // (A single fused warp-per-world kernel for the whole step would spread its warps
 // over every phase of a large instruction footprint, and the light phases would
 // inherit the narrowphase's register count and occupancy.)
@@ -2465,10 +2565,12 @@ __device__ __forceinline__ void forEachWorldBody(const EngineState &S, const Phy
     }
 }
 
-// One warp per world; kPhysWarps worlds per block.  (Fusing neighbouring phases
-// into one launch -- integrate -> narrowphase, position solve -> velocity update
-// -> velocity solve -- was measured: no gain, and the bigger kernels miss the
-// 32 KB instruction cache more; see DESIGN.md 3.2.)
+// kPhysWarps warps per block: one world per warp in the candidate search, 32 /
+// kSolverLanes worlds per warp in the solves.  physicsHostAfterRegistry sets
+// the position solve's carveout to the maximum shared memory for its body stage.  (Fusing neighbouring phases into one
+// launch -- integrate -> narrowphase, position solve -> velocity update ->
+// velocity solve -- was measured without staging: no gain, and the bigger
+// kernels miss the 32 KB instruction cache more; see DESIGN.md 3.2.)
 #ifndef MB2_NARROW_MINB
 #define MB2_NARROW_MINB 8
 #endif
@@ -2491,12 +2593,14 @@ physWorldKernel(EngineState *Sp)
         const i32 my_w = (i32)((blockIdx.x * blockDim.x + threadIdx.x) / kSolverLanes);
         const bool valid = my_w < (i32)S.numWorlds;
         const i32 w = valid ? my_w : (i32)S.numWorlds - 1;
+        constexpr int kWorldsPerBlock = 32 * kPhysWarps / kSolverLanes;
         if constexpr (OP == PhaseSolvePositions) {
             // the hull queue of this substep has been consumed: empty it for the next one
             if (blockIdx.x == 0 && threadIdx.x == 0) *P.hullQueueCount = 0;
-            __shared__ i32 last_level[32 * kPhysWarps / kSolverLanes][kMaxLevelBodies];
+            __shared__ i32 last_level[kWorldsPerBlock][kMaxLevelBodies];
+            __shared__ PosBody pos_stage[kWorldsPerBlock][kStagedBodies];
             orderContacts<kSolverLanes>(S, P, w, valid, lane, last_level[threadIdx.x / kSolverLanes]);
-            phaseSolvePositions(S, P, w, valid, lane);
+            phaseSolvePositions(S, P, w, valid, lane, pos_stage[threadIdx.x / kSolverLanes]);
         } else {
             phaseSolveVelocities(S, P, w, valid, lane);
         }
@@ -2595,6 +2699,12 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::stri
         return false;
     }
     cudaMemcpy(ph->dPhys, &P, sizeof(PhysicsState), cudaMemcpyHostToDevice);
+    // the position solve's body stage: prefer shared memory over L1 (measured with this setting)
+    if (cudaFuncSetAttribute(physWorldKernel<PhaseSolvePositions>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                             (int)cudaSharedmemCarveoutMaxShared) != cudaSuccess) {
+        *err = "setting the position solve's shared-memory carveout failed";
+        return false;
+    }
     return true;
 }
 
