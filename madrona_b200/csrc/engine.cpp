@@ -621,7 +621,7 @@ static bool enqueueNode(Executor *ex, uint32_t node_idx, cudaStream_t s)
     default:
         if (r.kind >= NodePhysBroadphaseUpdate) {
             std::string err;
-            if (!physicsEnqueueNode(ex, r, s, &err)) {
+            if (!physicsEnqueueNodes(ex, &r, 1, s, &err)) {
                 setError(err);
                 return false;
             }

@@ -237,18 +237,6 @@ bool jitCompile(const std::vector<std::string> &sources,
         opts.push_back("-G");
     }
     for (const std::string &f : user_flags) opts.push_back(f);
-    // extra NVRTC options for A/B builds of the device headers, space separated
-    // (e.g. MADRONA_B200_JIT_DEFINES="-DMB2_TRACE_SEED=0")
-    if (const char *env = getenv("MADRONA_B200_JIT_DEFINES")) {
-        std::string all(env);
-        size_t at = 0;
-        while (at < all.size()) {
-            size_t end = all.find(' ', at);
-            if (end == std::string::npos) end = all.size();
-            if (end > at) opts.push_back(all.substr(at, end - at));
-            at = end + 1;
-        }
-    }
 
     // unity translation unit
     std::string unity =

@@ -839,13 +839,11 @@ __device__ __forceinline__ bool boxOutside(const float *lo, const float *hi, Vec
     return reach < 0.f;
 }
 
-#ifndef MB2_RAYCAST_MINB
-#define MB2_RAYCAST_MINB 3
-#endif
+constexpr int kRaycastMinBlocks = 3;   // blocks per SM the ray caster is compiled for
 // FLAT: this launch traces the views of worlds with <= kFlatInstances instances, the other
 // instantiation the rest (a view belongs to exactly one of the two launches)
 template <bool FLAT>
-__global__ void __launch_bounds__(256, MB2_RAYCAST_MINB)
+__global__ void __launch_bounds__(256, kRaycastMinBlocks)
 renderRaycastKernel(EngineState *Sp)
 {
     pdlSync();
@@ -1334,7 +1332,7 @@ LaunchGraph *physicsBuildRenderGraph(Executor *ex, std::string *err)
     // persistent blocks striding over the views (the output table's capacity can be far above
     // the live view count: one block per capacity row cost 76 us of empty-block scheduling at
     // 1024 worlds); 8 rounds of resident blocks keep the tail short
-    const unsigned view_blocks = (unsigned)std::max(1, std::min(R.maxViews, ex->numSMs * MB2_RAYCAST_MINB * 8));
+    const unsigned view_blocks = (unsigned)std::max(1, std::min(R.maxViews, ex->numSMs * kRaycastMinBlocks * 8));
     launchK(renderRaycastKernel<true>, dim3(1, view_blocks), dim3(256), 0, ex->stream, ex->dState);
     launchK(renderRaycastKernel<false>, dim3(1, view_blocks), dim3(256), 0, ex->stream, ex->dState);
     launchStatusCopy(ex, ex->stream);

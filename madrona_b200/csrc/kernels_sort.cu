@@ -32,10 +32,7 @@ namespace mb2 {
 
 constexpr int kSortThreads = 256;
 constexpr int kSortWarps = kSortThreads / 32;
-#ifndef MB2_SORT_ITEMS
-#define MB2_SORT_ITEMS 8
-#endif
-constexpr int kItemsPerThread = MB2_SORT_ITEMS;
+constexpr int kItemsPerThread = 8;
 constexpr int kTileItems = kSortThreads * kItemsPerThread;   // 2048
 constexpr int kMaxPasses = 4;
 
@@ -177,10 +174,7 @@ sortHistogramKernel(SortParams p)
 constexpr uint32_t kFlagAggregate = 1u << 30;
 constexpr uint32_t kFlagInclusive = 2u << 30;
 constexpr uint32_t kValueMask = (1u << 30) - 1u;
-#ifndef MB2_SORT_LOOK_WINDOW
-#define MB2_SORT_LOOK_WINDOW 8
-#endif
-constexpr int kLookWindow = MB2_SORT_LOOK_WINDOW;
+constexpr int kLookWindow = 8;
 
 __global__ void __launch_bounds__(kSortThreads, 4)
 sortOnesweepKernel(SortParams p, int pass)
@@ -847,23 +841,15 @@ void launchSortArchetype(Executor *ex, uint32_t archetype, int32_t col, cudaStre
 
     const int tiles = (t.capacity + kTileItems - 1) / kTileItems;
     const int hist_grid = std::max(1, std::min(tiles, ex->numSMs * 4));
-    // ticketed tiles: any grid size is deadlock free; more resident blocks hide the
+    // ticketed tiles: any grid size is deadlock free; 4 resident blocks per SM hide the
     // ranking / look-back latency of each tile
-    static const int sweep_per_sm = [] {
-        const char *v = getenv("MADRONA_B200_SWEEP_BLOCKS_PER_SM");
-        return (v && *v) ? std::max(1, atoi(v)) : 4;
-    }();
-    const int sweep_grid = std::max(1, std::min(tiles, ex->numSMs * sweep_per_sm));
+    const int sweep_grid = std::max(1, std::min(tiles, ex->numSMs * 4));
     launchK(sortHistogramKernel, dim3(hist_grid), dim3(kSortThreads), 0, s, p);
     for (int pass = 0; pass < p.numPasses; pass++) {
         launchK(sortOnesweepKernel, dim3(sweep_grid), dim3(kSortThreads), 0, s, p, pass);
     }
     const int rtiles = (t.capacity + kRearrangeTile - 1) / kRearrangeTile;
-    static const int move_per_sm = [] {
-        const char *v = getenv("MADRONA_B200_REARRANGE_BLOCKS_PER_SM");
-        return (v && *v) ? std::max(1, atoi(v)) : 8;
-    }();
-    const int rblocks = std::max(1, std::min(rtiles * std::max(1, t.numColumns / 2), ex->numSMs * move_per_sm));
+    const int rblocks = std::max(1, std::min(rtiles * std::max(1, t.numColumns / 2), ex->numSMs * 8));
     launchK(sortRearrangeKernel, dim3(rblocks), dim3(256), 0, s, p);
     const int row_blocks = std::max(1, std::min((t.capacity + 255) / 256, ex->numSMs * 4));
     dim3 rgrid((unsigned)row_blocks, (unsigned)t.numColumns);

@@ -11,7 +11,6 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *rc, std::st
 void physicsHostDestroy(Executor *ex);
 // reads device-side facts that select kernel variants; call before stream capture begins
 void physicsBeforeGraphCapture(Executor *ex);
-bool physicsEnqueueNode(Executor *ex, const NodeRecord &rec, cudaStream_t s, std::string *err);
 bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, cudaStream_t s,
                          std::string *err);
 LaunchGraph *physicsBuildRenderGraph(Executor *ex, std::string *err);

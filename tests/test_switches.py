@@ -1,12 +1,9 @@
 """Code paths kept behind switches for A/B measurements must stay correct: each runs the
 parity tests of the kernels it touches in a child process (the switches are read once per
-process / select a different JIT build).
+process).
 
   MADRONA_B200_SORT_FUSE_COPYBACK=1   copy-back of exported columns as work items of the
                                       rearrange kernel (default: separate launch, DESIGN 3.1)
-  MADRONA_B200_JIT_DEFINES=-DMB2_TRACE_MASK=0
-                                      BVH::traceRay as the one-phase ordered scan (default:
-                                      candidate mask + ordered re-test, device/madrona/physics.hpp)
 """
 import os
 import subprocess
@@ -19,8 +16,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CASES = {
     "fused_copy_back": ({"MADRONA_B200_SORT_FUSE_COPYBACK": "1"},
                         ["tests/test_sort_custom_key.py", "tests/test_gridworld.py"], None),
-    "trace_ray_one_phase_scan": ({"MADRONA_B200_JIT_DEFINES": "-DMB2_TRACE_MASK=0"},
-                                 ["tests/test_room.py"], "gpu_matches_golden"),
 }
 
 
