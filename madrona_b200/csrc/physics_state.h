@@ -82,18 +82,25 @@ struct PhysicsWorldParams {
 };
 
 // Role of phys::CandidateCollision (physics.hpp:52-57: two Locs + two primitive
-// indices, 24 B), packed to 16 B and extended with what the narrowphase would
-// otherwise look up again per contact:
-//   archPrim = aArch | bArch << 8 | aPrim << 16 | bPrim << 24
-//   slots    = aSlot | aMutable << 15 | ... same for b in the high half, i.e.
-//              ((slot << 1) | mutable) per side with slot = index of the body in
-//              its world's body list (0x7fff: unknown) and mutable = "writing the
-//              body back can change it" (see rotationIsNormalizeFixpoint).
-struct Candidate {
-    u32 archPrim;
+// indices, 24 B), resolved by the candidate search into everything about the pair
+// that stays fixed for the step, so that every substep's narrowphase only loads the
+// poses and the primitive boxes.  Side a / b are already in primitive type order
+// (sphere < hull < plane):
+//   aPrim, bPrim = indices into the world's ObjectManager::prims
+//   arch  = aArch | bArch << 8 | pair class << 16, class = aType | bType
+//           (1 sphere-sphere, 2 hull-hull, 3 sphere-hull, 5 sphere-plane, 6 hull-plane)
+//   slots = aSlot | aMutable << 15 | ... same for b in the high half, i.e.
+//           ((slot << 1) | mutable) per side with slot = index of the body in
+//           its world's body list (0x7fff: unknown) and mutable = "writing the
+//           body back can change it" (see rotationIsNormalizeFixpoint).
+struct alignas(16) Candidate {
+    u32 aPrim;
+    u32 bPrim;
     i32 aRow;
     i32 bRow;
+    u32 arch;
     u32 slots;
+    u32 pad[2];
 };
 
 struct HullQueueEntry {
@@ -169,7 +176,8 @@ struct PhysicsState {
     i32 *contactCounts;
     i32 *contactMaxLevel;        // [numWorlds]
     i32 maxContactsPerWorld;
-    // hull - hull candidates that passed the primitive-box test, any order
+    // the step's hull - hull candidates, any order: built by the candidate search,
+    // read by every substep's narrowphase (count reset before each search)
     HullQueueEntry *hullQueue;   // [numWorlds * maxCandidatesPerWorld]
     i32 *hullQueueCount;
 };
