@@ -71,9 +71,9 @@ typedef struct mb2_mesh_bvh_view {
 } mb2_mesh_bvh_view;
 
 typedef struct mb2_material_view {
-    void *textures;                /* cudaTextureObject_t *: textures are not sampled by this engine */
-    uint32_t num_texture_buffers;
-    void *texture_buffers;
+    void *textures;                /* cudaTextureObject_t * (device): sampled by the RGBD ray caster */
+    uint32_t num_texture_buffers;  /* entries of textures; a textureIdx at or above it fails the render */
+    void *texture_buffers;         /* cudaArray_t * (host), owned by whoever built the textures */
     void *materials;               /* madrona::Material * (device) or NULL */
 } mb2_material_view;
 
@@ -108,6 +108,38 @@ mb2_mesh_bvh_data *mb2_build_mesh_bvhs(const mb2_mesh_source *meshes, uint32_t n
 const void *mb2_mesh_bvh_data_view(const mb2_mesh_bvh_data *data, int device);
 const uint32_t *mb2_mesh_bvh_triangle_sources(const mb2_mesh_bvh_data *data);
 void mb2_mesh_bvh_data_destroy(mb2_mesh_bvh_data *data);
+
+/* Materials and textures -> render::MaterialData.  Role of
+ * render::AssetProcessor::initMaterialData (src/render/asset_processor.cpp):
+ * every texture becomes a cudaArray (uchar4, or BC7 blocks) behind a texture
+ * object with the reference's descriptor -- wrap on both axes, linear
+ * filtering, normalized float reads, normalized coordinates -- and the
+ * materials are uploaded as madrona::Material.  Every input is checked before
+ * the first CUDA call; on a bad one the call returns NULL and
+ * mb2_last_error() says why.  mb2_material_data_view returns the
+ * mb2_material_view that goes into mb2_render_config::material_data.  The
+ * executor adopts those pointers without owning them: destroy the handle
+ * (mb2_material_data_destroy: texture objects, arrays, device buffers) after
+ * every executor that uses it. */
+typedef struct mb2_source_texture {     /* == imp::SourceTexture */
+    const void *data;                   /* RGBA8 rows, or BC7 blocks in rows of width / 4 */
+    int32_t format;                     /* 0 R8G8B8A8, 1 BC7 (width, height multiples of 4) */
+    uint32_t width;
+    uint32_t height;
+    uint64_t num_bytes;                 /* width * height * 4, or width * height (BC7) */
+} mb2_source_texture;
+typedef struct mb2_source_material {    /* == imp::SourceMaterial */
+    float color[4];                     /* multiplies the texture's rgb */
+    int32_t texture_idx;                /* -1: no texture */
+    float roughness;
+    float metalness;
+} mb2_source_material;
+typedef struct mb2_material_data mb2_material_data;
+mb2_material_data *mb2_init_material_data(const mb2_source_material *materials, uint32_t num_materials,
+                                          const mb2_source_texture *textures, uint32_t num_textures,
+                                          int gpu_id);
+const mb2_material_view *mb2_material_data_view(const mb2_material_data *data);
+void mb2_material_data_destroy(mb2_material_data *data);
 
 /* MWCudaExecutor::initCUDA(int gpu_id), mw_gpu.hpp:122 / cuda_exec.cpp:2315.
  * Returns 0 on success. */

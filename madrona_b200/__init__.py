@@ -17,6 +17,7 @@ from .executor import (  # noqa: F401
     library_path,
     precompile,
     MeshBVHData,
+    MaterialData,
     RigidBodyAssets,
     PeerGather,
 )

@@ -69,6 +69,8 @@ static std::string describeErrors(uint32_t flags, uint32_t archetype)
     if (flags & ErrTooManyNodes) s += "too many taskgraph nodes ";
     if (flags & ErrRegistry) s += "ECS registration error (unregistered component, too many types, bad export slot) ";
     if (flags & ErrPhysicsOverflow) s += "physics buffer overflow ";
+    if (flags & ErrRenderAsset) s += "render asset error (a material's textureIdx is not below "
+        "materialData.numTextureBuffers; those pixels were shaded untextured) ";
     return s;
 }
 

@@ -212,6 +212,7 @@ enum ErrorFlags : u32 {
     ErrTooManyNodes = 1u << 4,
     ErrRegistry = 1u << 5,
     ErrPhysicsOverflow = 1u << 6,
+    ErrRenderAsset = 1u << 7,          // a material names a texture the render config does not have
 };
 
 #ifdef __CUDACC__

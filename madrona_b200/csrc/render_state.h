@@ -114,6 +114,11 @@ struct RenderState {
     // exportCountsGPU (src/render/ecs_system.cpp:317-348): totals of the last prepare
     u32 totalNumViews;
     u32 totalNumInstances;
+
+    // ---- host config: == materialData.textures / numTextureBuffers (device array of
+    // cudaTextureObject_t; materials with textureIdx >= numTextures raise ErrRenderAsset)
+    const unsigned long long *textures;
+    u32 numTextures;
 };
 
 }

@@ -42,6 +42,9 @@ EXPORTED_SYMBOLS = [
     "mb2_mesh_bvh_data_view",
     "mb2_mesh_bvh_triangle_sources",
     "mb2_mesh_bvh_data_destroy",
+    "mb2_init_material_data",
+    "mb2_material_data_view",
+    "mb2_material_data_destroy",
     "mb2_process_rigid_body_assets",
     "mb2_object_manager_ptr",
     "mb2_object_manager_host_assets",
@@ -148,6 +151,16 @@ class _MeshSourceC(ctypes.Structure):
     ]
 
 
+class _SourceTextureC(ctypes.Structure):    # == imp::SourceTexture
+    _fields_ = [("data", ctypes.c_void_p), ("format", ctypes.c_int32), ("width", ctypes.c_uint32),
+                ("height", ctypes.c_uint32), ("num_bytes", ctypes.c_uint64)]
+
+
+class _SourceMaterialC(ctypes.Structure):   # == imp::SourceMaterial
+    _fields_ = [("color", ctypes.c_float * 4), ("texture_idx", ctypes.c_int32),
+                ("roughness", ctypes.c_float), ("metalness", ctypes.c_float)]
+
+
 def library_path() -> str:
     # MADRONA_B200_LIB: an alternative build of the same library (A/B measurements)
     return os.environ.get("MADRONA_B200_LIB") or os.path.join(_PKG_DIR, "libmadrona_b200.so")
@@ -215,6 +228,13 @@ def load_library() -> ctypes.CDLL:
     lib.mb2_mesh_bvh_triangle_sources.restype = ctypes.POINTER(ctypes.c_uint32)
     lib.mb2_mesh_bvh_data_destroy.argtypes = [vp]
     lib.mb2_mesh_bvh_data_destroy.restype = None
+    lib.mb2_init_material_data.argtypes = [ctypes.POINTER(_SourceMaterialC), ctypes.c_uint32,
+                                           ctypes.POINTER(_SourceTextureC), ctypes.c_uint32, ctypes.c_int]
+    lib.mb2_init_material_data.restype = vp
+    lib.mb2_material_data_view.argtypes = [vp]
+    lib.mb2_material_data_view.restype = ctypes.POINTER(_MaterialViewC)
+    lib.mb2_material_data_destroy.argtypes = [vp]
+    lib.mb2_material_data_destroy.restype = None
     lib.mb2_process_rigid_body_assets.argtypes = [ctypes.POINTER(_SourceHullC), ctypes.c_uint32,
                                                   ctypes.POINTER(_SourceObjectC), ctypes.c_uint32, ctypes.c_int]
     lib.mb2_process_rigid_body_assets.restype = vp
@@ -491,18 +511,26 @@ class MeshBVHData:
     """BLAS of a set of triangle meshes in the reference's MeshBVHData format (role of
     render::AssetProcessor::makeBVHData): `view(device=True)` is what goes into
     CudaBatchRenderConfig.geoBVHData.  meshes: list of (positions [nv,3] f32, indices
-    [nt,3] u32, material_idx)."""
+    [nt,3] u32, material_idx) or (positions, indices, material_idx, uvs [nv,2] f32); meshes
+    without uvs get (0, 0) at every vertex."""
 
     def __init__(self, meshes, gpu_id: int = -1):
         import numpy as np
         self._lib = load_library()
         self._keep = []
         srcs = (_MeshSourceC * len(meshes))()
-        for i, (pos, idx, mat) in enumerate(meshes):
+        for i, mesh in enumerate(meshes):
+            pos, idx, mat = mesh[:3]
             pos = np.ascontiguousarray(pos, dtype=np.float32)
             idx = np.ascontiguousarray(idx, dtype=np.uint32)
-            self._keep += [pos, idx]
-            srcs[i] = _MeshSourceC(pos.ctypes.data, None, len(pos), idx.ctypes.data, len(idx), int(mat))
+            uvs = None
+            if len(mesh) > 3 and mesh[3] is not None:
+                uvs = np.ascontiguousarray(mesh[3], dtype=np.float32)
+                if uvs.shape != (len(pos), 2):
+                    raise MadronaB200Error(f"mesh {i}: uvs must be [{len(pos)}, 2], got {list(uvs.shape)}")
+            self._keep += [pos, idx, uvs]
+            srcs[i] = _MeshSourceC(pos.ctypes.data, None if uvs is None else uvs.ctypes.data, len(pos),
+                                   idx.ctypes.data, len(idx), int(mat))
         self.num_triangles = [len(m[1]) for m in meshes]
         self._h = self._lib.mb2_build_mesh_bvhs(srcs, len(meshes), gpu_id)
         if not self._h:
@@ -531,6 +559,58 @@ class MeshBVHData:
     def close(self):
         if self._h:
             self._lib.mb2_mesh_bvh_data_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class MaterialData:
+    """Materials and textures in the reference's MaterialData format (role of
+    render::AssetProcessor::initMaterialData): `view()` is what goes into
+    CudaBatchRenderConfig.materialData.
+
+    materials: list of (color rgba, texture_idx, roughness, metalness); texture_idx -1 = none.
+    textures:  list of (data, format, width, height) == imp::SourceTexture, data a bytes-like
+               buffer (RGBA8 rows, or BC7 16-byte blocks in rows of width / 4) or None.
+    Executors adopt the pointers without owning them: close this after every executor
+    that was created from it."""
+
+    R8G8B8A8 = 0
+    BC7 = 1
+
+    def __init__(self, materials, textures=(), gpu_id: int = 0):
+        import numpy as np
+        self._lib = load_library()
+        self._h = None
+        self._keep = []
+        c_tex = (_SourceTextureC * max(len(textures), 1))()
+        for i, (data, fmt, width, height) in enumerate(textures):
+            ptr, nbytes = None, 0
+            if data is not None:
+                buf = np.ascontiguousarray(np.frombuffer(memoryview(data).cast("B"), dtype=np.uint8))
+                self._keep.append(buf)
+                ptr, nbytes = buf.ctypes.data, buf.nbytes
+            c_tex[i] = _SourceTextureC(ptr, int(fmt), int(width), int(height), nbytes)
+        c_mat = (_SourceMaterialC * max(len(materials), 1))()
+        for i, (color, tex_idx, roughness, metalness) in enumerate(materials):
+            c_mat[i] = _SourceMaterialC((ctypes.c_float * 4)(*[float(c) for c in color]), int(tex_idx),
+                                        float(roughness), float(metalness))
+        self.num_textures = len(textures)
+        self._h = self._lib.mb2_init_material_data(c_mat, len(materials), c_tex, len(textures), int(gpu_id))
+        self._keep = None        # the pixels were copied to the device
+        if not self._h:
+            raise MadronaB200Error(_last_error(self._lib))
+
+    def view(self) -> _MaterialViewC:
+        return self._lib.mb2_material_data_view(self._h).contents
+
+    def close(self):
+        if self._h:
+            self._lib.mb2_material_data_destroy(self._h)
             self._h = None
 
     def __del__(self):

@@ -239,6 +239,23 @@ SIMS: Dict[str, SimDesc] = {
         render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_render_config(
             int(cfg.get("resolution", 40)), bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0))),
     ),
+    # GPU only: the gallery sim with uvs and textured materials (tests/test_render_textures.py);
+    # same sources and flags, so it shares the gallery's simulator module
+    "gallery_textured": SimDesc(
+        name="gallery_textured",
+        sources=[os.path.join(_ROOT, "gallery", "sim.cpp")],
+        num_exports=10,
+        num_taskgraphs=1,
+        inputs=[],
+        outputs=[],
+        pack_config=lambda cfg: struct.pack("<II", int(cfg["num_props"]), 5),
+        pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
+        oracle_extra=lambda cfg: [],
+        defaults={"num_props": 100, "seed": 0, "resolution": 40, "rgbd": True, "bc7": False},
+        render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_textured_render_config(
+            int(cfg.get("resolution", 40)), bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)),
+            bc7=bool(cfg.get("bc7", False))),
+    ),
     # GPU only: 145 bodies per world, past the per-world body cap (tests/test_cliffs.py)
     "balls_cliff": SimDesc(
         name="balls_cliff",

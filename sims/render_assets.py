@@ -135,3 +135,160 @@ GALLERY_MATERIALS[:, 4] = np.array([-1], dtype=np.int32).view(np.float32)[0]    
 
 def make_gallery_render_config(resolution: int, rgbd: bool, gpu_id: int = 0):
     return make_render_config_from_meshes(gallery_meshes(), resolution, rgbd, gpu_id, materials=GALLERY_MATERIALS)
+
+
+# ---- textured gallery: the same meshes with uvs, three generated textures -----------------------
+# Pixels are made in code (decoding image files is the importer's job).  Each texture is built to
+# catch one kind of mistake: the checker a wrong `1 - v` flip or barycentric order (8 x 8 with an
+# asymmetric tint), the gradient swapped width and height (64 x 32), and the BC7 one the
+# block-compressed upload path (mode-6 blocks, 16 x 16).
+
+BC7_MODE6_WEIGHTS = np.array([0, 4, 9, 13, 17, 21, 26, 30, 34, 38, 43, 47, 51, 55, 60, 64], dtype=np.int64)
+
+
+def _bc7_interp(e0, e1):
+    """[..., 16 weights, 4] palette of a mode-6 block from 8-bit endpoints [..., 4]."""
+    w = BC7_MODE6_WEIGHTS[:, None]
+    return ((64 - w) * e0[..., None, :] + w * e1[..., None, :] + 32) >> 6
+
+
+def bc7_mode6_encode(rgba):
+    """RGBA8 [H, W, 4] (H, W multiples of 4) -> BC7 blocks uint8 [H/4, W/4, 16], mode 6 only:
+    7-bit RGBA endpoints with one p-bit each, 4-bit indices.  The endpoints are the block's
+    extremes along its principal axis, quantised with the p-bit pair of least error; every
+    texel takes its nearest palette entry."""
+    img = np.asarray(rgba, dtype=np.int64)
+    H, W = img.shape[:2]
+    assert img.shape[2] == 4 and H % 4 == 0 and W % 4 == 0
+    out = np.zeros((H // 4, W // 4, 16), dtype=np.uint8)
+    for by in range(H // 4):
+        for bx in range(W // 4):
+            px = img[by * 4:by * 4 + 4, bx * 4:bx * 4 + 4].reshape(16, 4)
+            mean = px.mean(0)
+            axis = np.linalg.eigh(np.cov((px - mean).T) + 1e-9 * np.eye(4))[1][:, -1]
+            proj = (px - mean) @ axis
+            ends = np.clip([mean + proj.min() * axis, mean + proj.max() * axis], 0, 255)
+            best = None
+            for p0 in (0, 1):
+                for p1 in (0, 1):
+                    c0 = np.clip(np.round((ends[0] - p0) / 2), 0, 127).astype(np.int64)
+                    c1 = np.clip(np.round((ends[1] - p1) / 2), 0, 127).astype(np.int64)
+                    pal = _bc7_interp((c0 << 1) | p0, (c1 << 1) | p1)
+                    d = ((px[:, None, :] - pal[None]) ** 2).sum(-1)
+                    err = d.min(1).sum()
+                    if best is None or err < best[0]:
+                        best = (err, c0, c1, p0, p1, d.argmin(1))
+            _, c0, c1, p0, p1, idx = best
+            if idx[0] >= 8:           # the anchor index has 3 bits: swap the endpoints
+                c0, c1, p0, p1 = c1, c0, p1, p0
+                idx = 15 - idx
+            bits = 1 << 6             # mode 6
+            pos = 7
+            for ch in range(4):
+                for c in (c0, c1):
+                    bits |= int(c[ch]) << pos
+                    pos += 7
+            bits |= p0 << pos
+            bits |= p1 << (pos + 1)
+            pos += 2
+            for i in range(16):
+                bits |= int(idx[i]) << pos
+                pos += 3 if i == 0 else 4
+            assert pos == 128
+            out[by, bx] = np.frombuffer(bits.to_bytes(16, "little"), dtype=np.uint8)
+    return out
+
+
+def bc7_mode6_decode(blocks):
+    """BC7 mode-6 blocks uint8 [H/4, W/4, 16] -> RGBA8 [H, W, 4] (the format's exact decode)."""
+    blocks = np.asarray(blocks, dtype=np.uint8)
+    bh, bw = blocks.shape[:2]
+    out = np.zeros((bh * 4, bw * 4, 4), dtype=np.uint8)
+    for by in range(bh):
+        for bx in range(bw):
+            bits = int.from_bytes(blocks[by, bx].tobytes(), "little")
+            assert bits & 0x7F == 1 << 6, "not a mode-6 block"
+            pos = 7
+            c = np.zeros((2, 4), dtype=np.int64)
+            for ch in range(4):
+                for e in range(2):
+                    c[e, ch] = (bits >> pos) & 0x7F
+                    pos += 7
+            p = [(bits >> pos) & 1, (bits >> (pos + 1)) & 1]
+            pos += 2
+            pal = _bc7_interp((c[0] << 1) | p[0], (c[1] << 1) | p[1])
+            for i in range(16):
+                n = 3 if i == 0 else 4
+                out[by * 4 + i // 4, bx * 4 + i % 4] = pal[(bits >> pos) & ((1 << n) - 1)]
+                pos += n
+    return out
+
+
+def checker_texture():
+    """8 x 8 RGBA8 checker: dark cells, light cells tinted by column and row."""
+    i, j = np.meshgrid(np.arange(8), np.arange(8))          # i: column (u), j: row
+    light = np.stack([np.full((8, 8), 255), 255 - 24 * i, 255 - 24 * j, np.full((8, 8), 255)], -1)
+    dark = np.broadcast_to(np.array([16, 16, 40, 255]), (8, 8, 4))
+    return np.where(((i + j) % 2 == 0)[..., None], light, dark).astype(np.uint8)
+
+
+def gradient_texture():
+    """64 wide x 32 high smooth RGBA8 gradient."""
+    x, y = np.meshgrid(np.arange(64), np.arange(32))
+    return np.stack([np.round(255 * x / 63), np.round(255 * y / 31), np.round(60 + 3 * (x + y) / 2),
+                     np.full(x.shape, 255)], -1).astype(np.uint8)
+
+
+def bc7_source_image():
+    """16 x 16 RGBA8 image the BC7 texture is encoded from."""
+    x, y = np.meshgrid(np.arange(16), np.arange(16))
+    return np.stack([16 * x + 8, 255 - 12 * y, 128 + 7 * (x - y), np.full(x.shape, 255)], -1).astype(np.uint8)
+
+
+def gallery_textures():
+    """[(texels RGBA8 [H, W, 4] as sampled, format, source bytes)]: checker, gradient, BC7."""
+    bc7 = bc7_mode6_encode(bc7_source_image())
+    return [(checker_texture(), 0, checker_texture().tobytes()),
+            (gradient_texture(), 0, gradient_texture().tobytes()),
+            (bc7_mode6_decode(bc7), 1, bc7.tobytes())]
+
+
+def _planar_uvs(v, scale):
+    """uv linear in the position (no box face maps to a line), centred on 0.5."""
+    v = np.asarray(v, dtype=np.float64)
+    return np.stack([scale * (v[:, 0] + 0.5 * v[:, 2]) + 0.5, scale * (v[:, 1] - 0.5 * v[:, 2]) + 0.5],
+                    1).astype(np.float32)
+
+
+def gallery_textured_meshes():
+    """gallery_meshes() with uvs: props mapped planar (uvs about [-1, 2], so they wrap), the
+    ground quad's corners at uv 0 and 6."""
+    out = []
+    for k, (v, f, mat) in enumerate(gallery_meshes()):
+        if k == 4:
+            uv = np.array([[0, 0], [6, 0], [6, 6], [0, 6]], dtype=np.float32)
+        else:
+            uv = _planar_uvs(v, 1.5)
+        out.append((v, f, mat, uv))
+    return out
+
+
+def gallery_textured_materials(bc7: bool = False):
+    """GALLERY_MATERIALS' colours; material 0 (the ground's override) samples the checker,
+    material 2 (the icosphere's default) the gradient, or with bc7 the BC7 texture."""
+    tex_of = {0: 0, 2: 2 if bc7 else 1}
+    return [(tuple(float(c) for c in m[:4]), tex_of.get(i, -1), float(m[5]), float(m[6]))
+            for i, m in enumerate(GALLERY_MATERIALS)]
+
+
+def make_gallery_textured_render_config(resolution: int, rgbd: bool, gpu_id: int = 0, bc7: bool = False):
+    """CudaBatchRenderConfig with textured materials uploaded by mb2_init_material_data; the
+    MaterialData in keep_alive must outlive the executor."""
+    import madrona_b200 as mb
+    from madrona_b200.executor import _RenderConfigC
+
+    bvh = mb.MeshBVHData(gallery_textured_meshes(), gpu_id=gpu_id)
+    textures = [(src, fmt, t.shape[1], t.shape[0]) for t, fmt, src in gallery_textures()]
+    mats = mb.MaterialData(gallery_textured_materials(bc7), textures, gpu_id=gpu_id)
+    rc = _RenderConfigC(0 if rgbd else 1, bvh.view(device=True), mats.view(), resolution, 0.001, 1000.0)
+    return rc, [bvh, mats]
