@@ -468,10 +468,13 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
         if (!resetForInitPass(ex, 0, {}, persist_mark)) return false;
         if (!launch1(ex, ex->initWorlds, wblocks, 128)) return false;
         // a dynamic table too small for the worlds' initial population: double it and
-        // construct again (the dry run exists to be repeated)
+        // construct again (the dry run exists to be repeated).  The entity store is sized
+        // from the table capacities, so a large overflow exhausts it too; growTable grows
+        // it along with the table.
         uint32_t st[2] = { 0, 0 };
         MB2_CUDA(cudaMemcpy(st, &ex->dState->errorFlags, sizeof(st), cudaMemcpyDeviceToHost));
-        if (st[0] == (uint32_t)ErrTableOverflow && ex->tableGrowth && attempt < 12 &&
+        const bool table_overflow = (st[0] & ~(uint32_t)ErrEntityOverflow) == (uint32_t)ErrTableOverflow;
+        if (table_overflow && ex->tableGrowth && attempt < 12 &&
                 st[1] < S.numArchetypes && !ex->columnRanges[st[1]].empty()) {
             std::string gerr;
             if (!growTable(ex, st[1], (int64_t)S.tables[st[1]].capacity * 2, &gerr)) {

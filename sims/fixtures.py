@@ -104,6 +104,32 @@ SIMS: Dict[str, SimDesc] = {
         oracle_extra=lambda cfg: [],
         defaults={"items_per_world": 9, "key_mask": 0xFFFFFFFF, "seed": 0},
     ),
+    # GPU only: sort / compaction at tile, pass and column-width edges (tests/test_sort_sweep.py);
+    # per-world lists init_counts / creates / kill_steps (kill step 0 = never)
+    "sortsweep": SimDesc(
+        name="sortsweep",
+        sources=[os.path.join(_ROOT, "sortsweep", "sim.cpp")],
+        num_exports=10,
+        num_taskgraphs=1,
+        inputs=[],
+        outputs=[Slot(0, "entity", "int32", (2,), dynamic=True),
+                 Slot(1, "uid", "uint32", (1,), dynamic=True),
+                 Slot(2, "key4", "uint32", (1,), dynamic=True),
+                 Slot(3, "check", "uint32", (1,), dynamic=True),
+                 Slot(4, "p2", "uint8", (2,), dynamic=True),
+                 Slot(5, "p3", "uint8", (3,), dynamic=True),
+                 Slot(6, "p12", "uint8", (12,), dynamic=True),
+                 Slot(7, "p24", "uint8", (24,), dynamic=True),
+                 Slot(8, "p48", "uint8", (48,), dynamic=True),
+                 Slot(9, "summary", "uint32", (2,))],
+        pack_config=lambda cfg: struct.pack("<IIII", int(cfg["shape"]), int(cfg["key_mode"]),
+                                            int(cfg["sort_on_key8"]), int(cfg["destroy_threshold"])),
+        pack_init=lambda w, cfg: struct.pack("<IIII", int(cfg.get("seed", 0)) + w, int(cfg["init_counts"][w]),
+                                             int(cfg["creates"][w]), int(cfg["kill_steps"][w])),
+        oracle_extra=lambda cfg: [],
+        defaults={"shape": 0, "key_mode": 0, "sort_on_key8": 0, "destroy_threshold": 0, "seed": 0,
+                  "init_counts": [9], "creates": [0], "kill_steps": [0]},
+    ),
     "room": SimDesc(
         name="room",
         sources=[os.path.join(_ROOT, "room", "sim.cpp")],

@@ -4,6 +4,8 @@ process).
 
   MADRONA_B200_SORT_FUSE_COPYBACK=1   copy-back of exported columns as work items of the
                                       rearrange kernel (default: separate launch, DESIGN 3.1)
+  MADRONA_B200_PDL=1                  programmatic dependent launch of every engine kernel:
+                                      each must reach pdlSync() before it touches memory
 """
 import os
 import subprocess
@@ -15,7 +17,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 CASES = {
     "fused_copy_back": ({"MADRONA_B200_SORT_FUSE_COPYBACK": "1"},
-                        ["tests/test_sort_custom_key.py", "tests/test_gridworld.py"], None),
+                        ["tests/test_sort_sweep.py", "tests/test_sort_custom_key.py", "tests/test_gridworld.py"],
+                        None),
+    "pdl": ({"MADRONA_B200_PDL": "1"},
+            ["tests/test_sort_sweep.py", "tests/test_sort_custom_key.py", "tests/test_gridworld.py",
+             "tests/test_room.py"], None),
 }
 
 
