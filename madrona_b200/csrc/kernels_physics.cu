@@ -78,6 +78,7 @@ struct PhysicsHost {
     PhysicsState hPhys;
     bool active = false;
     bool spheres = false;     // some registered object has a sphere primitive (read before graph capture)
+    unsigned narrowBlocks = 0;   // persistent narrowphase grid for that kernel (0: occupancy query failed)
 };
 
 // ---- small device helpers ------------------------------------------------------------
@@ -686,17 +687,23 @@ __device__ void phaseFindCandidates(EngineState &S, const PhysicsState &P, const
     }
     if (lane == 0) P.candCounts[w] = running;
 
-    // the step's hull - hull work list (one atomic per warp and 32 candidates)
+    // the step's two work lists, hull - hull pairs and the others (one atomic per
+    // warp, list and 32 candidates)
     __syncwarp();
     for (i32 base = 0; base < running; base += 32) {
         const i32 i = base + lane;
-        const bool hh = i < running && (out[i].arch >> 16) == 2u;
-        const unsigned mask = __ballot_sync(0xffffffffu, hh);
-        if (!mask) continue;
-        i32 at = 0;
-        if (lane == 0) at = atomicAdd(P.hullQueueCount, __popc(mask));
-        at = __shfl_sync(0xffffffffu, at, 0);
-        if (hh) P.hullQueue[at + __popc(mask & ((1u << lane) - 1u))] = HullQueueEntry { w, i };
+        const bool valid = i < running;
+        const bool hh = valid && (out[i].arch >> 16) == 2u;
+        const unsigned hh_mask = __ballot_sync(0xffffffffu, hh);
+        const unsigned other_mask = __ballot_sync(0xffffffffu, valid && !hh);
+        i32 hh_at = 0, other_at = 0;
+        if (lane == 0 && hh_mask) hh_at = atomicAdd(&P.pairCounts[0], __popc(hh_mask));
+        if (lane == 0 && other_mask) other_at = atomicAdd(&P.pairCounts[1], __popc(other_mask));
+        hh_at = __shfl_sync(0xffffffffu, hh_at, 0);
+        other_at = __shfl_sync(0xffffffffu, other_at, 0);
+        const unsigned below = (1u << lane) - 1u;
+        if (hh) P.hullPairs[hh_at + __popc(hh_mask & below)] = PairEntry { w, i };
+        else if (valid) P.otherPairs[other_at + __popc(other_mask & below)] = PairEntry { w, i };
     }
 }
 
@@ -1572,93 +1579,108 @@ __device__ bool hullHullGroup(EngineState &S, const PairSetup &ps, HullScratch &
 
 // ---- narrowphase, dense over the candidates of ALL worlds ------------------------------------
 // The contact of candidate i of world w lives in slot (w, i), so nothing here
-// needs per-world ordering.  One launch per substep, one group per pair, blocks
-// split by pair class so neither class waits for the other:
-//   blocks [0, hull_blocks)   kGroupLanes-lane groups stride over the step's hull - hull
-//       list (built by the candidate search), the long chains first;
-//   the blocks after that     kPlaneLanes-lane groups over the candidates of
-//       kNarrowWorldsPerBlock worlds, their lists flattened (groups stay busy whatever
-//       the per-world counts are): every pair but hull - hull;
-//   orderContacts (prologue of the position solve) lists each world's hits in
-//       candidate order and assigns the dependency levels.
-// Each class writes candHit for its own slots.
-constexpr int kNarrowThreads = 64;
-constexpr int kNarrowGroups = kNarrowThreads / kGroupLanes;
-// blocks/SM: the most that compile without local memory (91 / 128 registers)
-constexpr int kNarrowMinBlocks = 10;
-constexpr int kNarrowMinBlocksSpheres = 8;
+// needs per-world ordering.  One launch per substep, a persistent grid of
+// numSMs x (resident blocks per SM) blocks over the step's two work lists (built
+// by the candidate search).  The unit of work is a warp item: kGroupLanes-lane
+// groups on 4 hull - hull pairs, or kPlaneLanes-lane groups on 8 other pairs.
+// Items are numbered [hull - hull items][other items], so the long chains start
+// first, and handed out in that order by a ticket (one atomic per warp and item,
+// fetched while the previous item runs): both classes share every SM, neither
+// waits for a wave of the other, and a warp that drew short pairs takes more.
+// Each pair writes only its own contact slot and candHit entry, so which warp
+// takes which pair changes no result.  orderContacts (prologue of the position
+// solve) lists each world's hits in candidate order and assigns the dependency
+// levels.
+// Threads per block, measured on an H100 80GB HBM3 at a 700 W power limit (bench.py
+// --steps 200 --warmup 20, means of 3 alternating runs, room / arena / room_render):
+// 128 threads 1.3276 / 1.5689 / 10.983 ms/step, of which phys_narrowphase 0.347 /
+// 0.295 / 0.622 ms; 64 threads 1.3284 / 1.5714 / 10.979 ms/step, phys_narrowphase
+// 0.349 / 0.296 / 0.627 ms.
+constexpr int kNarrowThreads = 128;
+constexpr int kNarrowWarps = kNarrowThreads / 32;
+// 640 / 512 resident threads per SM: the most that compile without local memory
+// (96 / 128 registers)
+constexpr int kNarrowMinBlocks = 640 / kNarrowThreads;
+constexpr int kNarrowMinBlocksSpheres = 512 / kNarrowThreads;
 // Lanes per hull - plane pair.  Measured on an H100 80GB HBM3 at a 400 W power limit
 // (bench.py --steps 200, ms/step, room / arena / room_render): 4 lanes 1.376 / 1.596 /
 // 11.66, 8 lanes 1.479 / 1.713 / 11.85.  With 2 lanes or 1 the room step took
 // 2.0 / 1.9 ms.
 constexpr int kPlaneLanes = 4;
-constexpr int kPlaneGroups = kNarrowThreads / kPlaneLanes;
-constexpr int kNarrowWorldsPerBlock = 2;
+constexpr int kHullPairsPerWarp = 32 / kGroupLanes;
+constexpr int kPlanePairsPerWarp = 32 / kPlaneLanes;
 
 template <bool SPHERE_HULL>
 __global__ void __launch_bounds__(kNarrowThreads, SPHERE_HULL ? kNarrowMinBlocksSpheres : kNarrowMinBlocks)
-physNarrowphaseKernel(EngineState *Sp, u32 hull_blocks)
+physNarrowphaseKernel(EngineState *Sp)
 {
     pdlSync();
     EngineState &S = *Sp;
     const PhysicsState &P = *S.physics;
     fillColCache(S, P);
-    // hull - hull blocks and the other blocks use their own part of the same shared memory
+    // per warp: the scratch of its 4 hull - hull groups or of its 8 other groups
     __shared__ union {
-        HullScratch hull[kNarrowGroups];
-        PlaneScratch plane[kPlaneGroups];
-    } scratch;
+        HullScratch hull[kHullPairsPerWarp];
+        PlaneScratch plane[kPlanePairsPerWarp];
+    } scratch[kNarrowWarps];
     const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x / 32;
+    const i32 num_hull = P.pairCounts[0], num_other = P.pairCounts[1];
+    const i32 hull_items = (num_hull + kHullPairsPerWarp - 1) / kHullPairsPerWarp;
+    const i32 items = hull_items + (num_other + kPlanePairsPerWarp - 1) / kPlanePairsPerWarp;
+    i32 *const ticket = &P.pairCounts[2];
+    i32 item = 0;
+    if (lane == 0) item = atomicAdd(ticket, 1);
+    item = __shfl_sync(0xffffffffu, item, 0);
 
-    if (blockIdx.x < hull_blocks) {
+    while (item < hull_items) {
+        i32 next = 0;
+        if (lane == 0) next = atomicAdd(ticket, 1);    // in flight while this item runs
         const int sub = lane % kGroupLanes;
-        const int group = threadIdx.x / kGroupLanes;
-        const unsigned gm = ((1u << kGroupLanes) - 1u) << (lane / kGroupLanes * kGroupLanes);
-        const i32 count = *P.hullQueueCount;
-        for (i32 e = (i32)blockIdx.x * kNarrowGroups + group; e < count; e += (i32)hull_blocks * kNarrowGroups) {
-            const HullQueueEntry ent = P.hullQueue[e];
+        const int group = lane / kGroupLanes;
+        const unsigned gm = ((1u << kGroupLanes) - 1u) << (group * kGroupLanes);
+        const i32 e = item * kHullPairsPerWarp + group;
+        if (e < num_hull) {
+            const PairEntry ent = P.hullPairs[e];
             const size_t slot = (size_t)ent.world * P.maxCandidatesPerWorld + ent.cand;
             const PairSetup ps = setupPair(worldObjects(S, P, ent.world), P.candidates[slot]);
-            const bool made = ps.test != 0 && hullHullGroup(S, ps, scratch.hull[group], gm, sub, P.contacts[slot]);
+            const bool made = ps.test != 0 && hullHullGroup(S, ps, scratch[warp].hull[group], gm, sub,
+                                                             P.contacts[slot]);
             if (sub == 0) P.candHit[slot] = made ? 1 : 0;
-            __syncwarp(gm);
         }
-        return;
+        // the warp's next item may use its scratch in the other layout
+        __syncwarp();
+        item = __shfl_sync(0xffffffffu, next, 0);
     }
-
-    __shared__ i32 first[kNarrowWorldsPerBlock + 1];
-    const i32 w0 = (i32)(blockIdx.x - hull_blocks) * kNarrowWorldsPerBlock;
-    if (threadIdx.x == 0) {
-        i32 acc = 0;
-        for (int k = 0; k < kNarrowWorldsPerBlock; k++) {
-            first[k] = acc;
-            if (w0 + k < (i32)S.numWorlds) acc += P.candCounts[w0 + k];
+    while (item < items) {
+        i32 next = 0;
+        if (lane == 0) next = atomicAdd(ticket, 1);
+        const int sub = lane % kPlaneLanes;
+        const int group = lane / kPlaneLanes;
+        const unsigned gm = ((1u << kPlaneLanes) - 1u) << (group * kPlaneLanes);
+        const i32 e = (item - hull_items) * kPlanePairsPerWarp + group;
+        if (e < num_other) {
+            const PairEntry ent = P.otherPairs[e];
+            const size_t slot = (size_t)ent.world * P.maxCandidatesPerWorld + ent.cand;
+            const PairSetup ps = setupPair(worldObjects(S, P, ent.world), P.candidates[slot]);
+            bool made = false;
+            if (ps.test == 6) {
+                made = hullPlaneGroup<kPlaneLanes>(S, ps, scratch[warp].plane[group], gm, sub, P.contacts[slot]);
+            } else if (ps.test != 0) {
+                i32 hit = 0;
+                if (sub == 0) hit = singlePointPair<SPHERE_HULL>(S, ps, P.contacts[slot]) ? 1 : 0;
+                made = __shfl_sync(gm, hit, __ffs(gm) - 1) != 0;
+            }
+            if (sub == 0) P.candHit[slot] = made ? 1 : 0;
         }
-        first[kNarrowWorldsPerBlock] = acc;
+        __syncwarp();
+        item = __shfl_sync(0xffffffffu, next, 0);
     }
-    __syncthreads();
-    const i32 total = first[kNarrowWorldsPerBlock];
-    const int sub = lane % kPlaneLanes;
-    const int group = threadIdx.x / kPlaneLanes;
-    const unsigned gm = ((1u << kPlaneLanes) - 1u) << (lane / kPlaneLanes * kPlaneLanes);
-    for (i32 j = group; j < total; j += kPlaneGroups) {
-        int k = 0;
-        while (j >= first[k + 1]) k++;
-        const i32 w = w0 + k;
-        const size_t slot = (size_t)w * P.maxCandidatesPerWorld + (j - first[k]);
-        const Candidate cand = P.candidates[slot];
-        if ((cand.arch >> 16) == 2u) continue;          // hull - hull: the other blocks' pair
-        const PairSetup ps = setupPair(worldObjects(S, P, w), cand);
-        bool made = false;
-        if (ps.test == 6) {
-            made = hullPlaneGroup<kPlaneLanes>(S, ps, scratch.plane[group], gm, sub, P.contacts[slot]);
-        } else if (ps.test != 0) {
-            i32 hit = 0;
-            if (sub == 0) hit = singlePointPair<SPHERE_HULL>(S, ps, P.contacts[slot]) ? 1 : 0;
-            made = __shfl_sync(gm, hit, __ffs(gm) - 1) != 0;
-        }
-        if (sub == 0) P.candHit[slot] = made ? 1 : 0;
-        __syncwarp(gm);
+    // Every warp has taken its last ticket before it counts itself out, so the last
+    // one out can zero the ticket for the next launch.
+    if (lane == 0 && atomicAdd(&P.pairCounts[3], 1) == (i32)gridDim.x * kNarrowWarps - 1) {
+        P.pairCounts[2] = 0;
+        P.pairCounts[3] = 0;
     }
 }
 
@@ -2464,8 +2486,9 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::stri
         !alloc((void **)&P.contacts, sizeof(Contact) * W * P.maxCandidatesPerWorld) ||
         !alloc((void **)&P.candHit, sizeof(i32) * W * P.maxCandidatesPerWorld) ||
         !alloc((void **)&P.contactOrder, sizeof(i32) * W * P.maxContactsPerWorld) ||
-        !alloc((void **)&P.hullQueue, sizeof(HullQueueEntry) * W * P.maxCandidatesPerWorld) ||
-        !alloc((void **)&P.hullQueueCount, sizeof(i32) * 4) ||
+        !alloc((void **)&P.hullPairs, sizeof(PairEntry) * W * P.maxCandidatesPerWorld) ||
+        !alloc((void **)&P.otherPairs, sizeof(PairEntry) * W * P.maxCandidatesPerWorld) ||
+        !alloc((void **)&P.pairCounts, sizeof(i32) * 4) ||
         !alloc((void **)&P.contactCounts, sizeof(i32) * W) ||
         !alloc((void **)&P.contactMaxLevel, sizeof(i32) * W)) {
         *err = "physics buffers allocation failed";
@@ -2488,6 +2511,13 @@ void physicsBeforeGraphCapture(Executor *ex)
     u32 flag = 0;
     cudaMemcpy(&flag, &ph->dPhys->hasSpherePrims, sizeof(u32), cudaMemcpyDeviceToHost);
     ph->spheres = flag != 0;
+    // the narrowphase grid is exactly what is resident at once
+    int per_sm = 0;
+    const cudaError_t e = ph->spheres
+        ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, physNarrowphaseKernel<true>, kNarrowThreads, 0)
+        : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, physNarrowphaseKernel<false>, kNarrowThreads, 0);
+    if (e != cudaSuccess) cudaGetLastError();
+    ph->narrowBlocks = e == cudaSuccess ? (unsigned)ex->numSMs * (unsigned)per_sm : 0u;
 }
 
 void physicsHostDestroy(Executor *ex)
@@ -2536,20 +2566,20 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
             // joints are iterated per world by the solver: keep their table in
             // world order (the reference sorts Joint here too, xpbd.cpp:1092-1096)
             launchSortArchetype(ex, ph->hPhys.jointArchetype, 1, s);
-            // the search appends the step's hull - hull pairs to an empty list
-            cudaMemsetAsync(ph->hPhys.hullQueueCount, 0, sizeof(i32), s);
+            // the search appends the step's pairs to two empty lists
+            cudaMemsetAsync(ph->hPhys.pairCounts, 0, 2 * sizeof(i32), s);
             launchK(physFindCandidatesKernel, dim3(wgrid), dim3(wblock), 0, s, d);
             break;
         case NodePhysSubstepBegin:
             launchK(physBodyKernel<PhaseIntegrate>, dim3(bgrid), dim3(256), 0, s, d);
             break;
         case NodePhysNarrowphase:
-            {
-                const unsigned hull_blocks = (unsigned)ex->numSMs * (unsigned)kNarrowMinBlocks;
-                const dim3 grid(hull_blocks + (W + kNarrowWorldsPerBlock - 1) / kNarrowWorldsPerBlock);
-                if (ph->spheres) launchK(physNarrowphaseKernel<true>, grid, dim3(kNarrowThreads), 0, s, d, hull_blocks);
-                else launchK(physNarrowphaseKernel<false>, grid, dim3(kNarrowThreads), 0, s, d, hull_blocks);
+            if (ph->narrowBlocks == 0) {
+                *err = "narrowphase occupancy query failed";
+                return false;
             }
+            if (ph->spheres) launchK(physNarrowphaseKernel<true>, dim3(ph->narrowBlocks), dim3(kNarrowThreads), 0, s, d);
+            else launchK(physNarrowphaseKernel<false>, dim3(ph->narrowBlocks), dim3(kNarrowThreads), 0, s, d);
             break;
         case NodePhysSolvePositions:
             launchK(physSolvePositionsKernel, dim3(sgrid), dim3(wblock), 0, s, d);

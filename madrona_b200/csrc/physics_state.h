@@ -103,7 +103,7 @@ struct alignas(16) Candidate {
     u32 pad[2];
 };
 
-struct HullQueueEntry {
+struct PairEntry {
     i32 world;
     i32 cand;
 };
@@ -176,10 +176,14 @@ struct PhysicsState {
     i32 *contactCounts;
     i32 *contactMaxLevel;        // [numWorlds]
     i32 maxContactsPerWorld;
-    // the step's hull - hull candidates, any order: built by the candidate search,
-    // read by every substep's narrowphase (count reset before each search)
-    HullQueueEntry *hullQueue;   // [numWorlds * maxCandidatesPerWorld]
-    i32 *hullQueueCount;
+    // the step's candidates as two work lists, hull - hull pairs and all other pairs,
+    // in any order across worlds: built by the candidate search, read by every
+    // substep's narrowphase (counts reset before each search)
+    PairEntry *hullPairs;        // [numWorlds * maxCandidatesPerWorld]
+    PairEntry *otherPairs;       // [numWorlds * maxCandidatesPerWorld]
+    // [0] hull - hull, [1] other; [2], [3] the narrowphase's item ticket and
+    // finished-warp count, zero between launches
+    i32 *pairCounts;
 };
 
 }
