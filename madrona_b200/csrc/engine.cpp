@@ -669,6 +669,23 @@ static LaunchGraph *buildGraph(Executor *ex, const uint32_t *ids, uint32_t n, co
             ok = false;
             break;
         }
+        // The standalone overlap rows and a solver step do not mix, in one task graph or
+        // in two of the simulator's: the reference's solver would consume and clear the
+        // rows, while this engine's solver never materialises its candidates as rows, so
+        // the results would silently differ.
+        bool has_overlaps = false, has_solver = false;
+        for (uint32_t node = 0; node < S.numNodes; node++) {
+            const uint32_t kind = S.nodes[node].kind;
+            has_overlaps |= kind == NodePhysEmitOverlaps;
+            has_solver |= kind == NodePhysSubstepBegin || kind == NodePhysTGSVelocities;
+        }
+        if (has_overlaps && has_solver) {
+            setError("the simulator's task graphs contain both "
+                     "PhysicsSystem::setupStandaloneBroadphaseOverlapTasks and setupPhysicsStepTasks; "
+                     "the standalone overlap tasks are for simulators without the solver");
+            ok = false;
+            break;
+        }
         const size_t first_unit_of_graph = units.size();
         for (uint32_t node = 0; node < S.numNodes; node++) {
             if (S.nodes[node].taskgraph != ids[i]) continue;

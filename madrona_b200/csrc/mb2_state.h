@@ -127,6 +127,9 @@ enum NodeKind : u32 {
     NodePhysClearCandidates = 25,
     NodePhysTGSVelocities = 26,    // tgs::integrateVelocities (src/physics/tgs.cpp:92-142)
     NodePhysTGSPositions = 27,     // tgs::integratePositions (tgs.cpp:171-195)
+    // the candidate list as CandidateCollision rows of the CandidateTemporary table
+    // (PhysicsSystem::setupStandaloneBroadphaseOverlapTasks, broadphase.cpp:930-993)
+    NodePhysEmitOverlaps = 28,
     NodeRenderPrepare = 32,
 };
 

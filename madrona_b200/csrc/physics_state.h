@@ -93,6 +93,11 @@ struct PhysicsWorldParams {
 //           ((slot << 1) | mutable) per side with slot = index of the body in
 //           its world's body list (0x7fff: unknown) and mutable = "writing the
 //           body back can change it" (see rotationIsNormalizeFixpoint).
+//   pad[0] = the pair as the reference's CandidateCollision row has it, for the
+//           standalone overlap rows (NodePhysEmitOverlaps): aRel | bRel << 8 |
+//           swapped << 16, with aRel / bRel the primitive indices within the
+//           iterating body (smaller entity ID) and its partner, and swapped set
+//           when side a above is the partner (primitive type order reversed it)
 struct alignas(16) Candidate {
     u32 aPrim;
     u32 bPrim;

@@ -62,6 +62,15 @@ struct CandidateCollision {
     uint32_t bPrim;
 };
 
+namespace impl {
+
+// == CandidateTemporary (src/physics/physics_impl.hpp:17): the rows of
+// setupStandaloneBroadphaseOverlapTasks.  Engine-private like the reference's;
+// simulator code reaches the rows through a CandidateCollision query.
+struct CandidateTemporary : Archetype<CandidateCollision> {};
+
+}
+
 struct ContactConstraint {
     Loc ref;
     Loc alt;
@@ -243,6 +252,9 @@ inline void registerTypes(ECSRegistry &registry, Solver solver = Solver::XPBD)
     registry.registerArchetype<CollisionEventTemporary>();
 
     registry.registerComponent<CandidateCollision>();
+    // a temporary archetype, no singleton: entity IDs stay those of the CPU backend
+    registry.registerArchetype<impl::CandidateTemporary>();
+
     registry.registerComponent<JointConstraint>();
     registry.registerComponent<ContactConstraint>();
 
@@ -454,6 +466,100 @@ inline TaskGraphNodeID setupCleanupTasks(TaskGraphBuilder &builder,
                                          Span<const TaskGraphNodeID> deps)
 {
     return builder.addToGraph<ClearTmpNode<CollisionEventTemporary>>(deps);
+}
+
+// Broadphase without the solver (reference: physics.cpp:393-405): after
+// setupBroadphaseTasks, the candidate search lists every overlapping primitive
+// pair of each world and the engine writes them as CandidateCollision rows --
+// a = the body with the smaller entity ID, aPrim / bPrim = primitive indices
+// within each body, each world's rows in the CPU backend's order -- for user
+// systems to query.  The rows replace the table's previous contents; the
+// cleanup task clears them.  A task graph may not also contain
+// setupPhysicsStepTasks (rejected when its launch graph is built).
+inline TaskGraphNodeID setupStandaloneBroadphaseOverlapTasks(TaskGraphBuilder &builder,
+                                                             Span<const TaskGraphNodeID> deps)
+{
+    // tag 1: no solver follows, the Joint table needs no world sort
+    TaskGraphNodeID cur = mwGPU::pushBuiltin(builder, deps, mb2::NodePhysFindCandidates, 0, 0, 1);
+    return mwGPU::pushBuiltin(builder, { cur }, mb2::NodePhysEmitOverlaps,
+                              TypeTracker::typeID<impl::CandidateTemporary>(),
+                              TypeTracker::typeID<CandidateCollision>());
+}
+
+inline TaskGraphNodeID setupStandaloneBroadphaseCleanupTasks(TaskGraphBuilder &builder,
+                                                             Span<const TaskGraphNodeID> deps)
+{
+    return builder.addToGraph<ClearTmpNode<impl::CandidateTemporary>>(deps);
+}
+
+// Does any HULL primitive of e overlap aabb (reference: physics.cpp:159-252)?
+// Per primitive: its transformed box must overlap aabb, then the hull's
+// vertices rot * (scale * v) + pos are projected onto the x, y and z axes and
+// both intervals must overlap strictly on all three.  Sphere and plane
+// primitives never count, as in the reference.  An entity that no longer
+// exists overlaps nothing.
+inline bool checkEntityAABBOverlap(Context &ctx, math::AABB aabb, Entity e)
+{
+    using namespace math;
+    if (!ctx.loc(e).valid()) return false;
+    const ObjectManager &obj_mgr = *ctx.singleton<ObjectData>().mgr;
+
+    const base::ObjectID e_obj_id = ctx.get<base::ObjectID>(e);
+    const Vector3 e_pos = ctx.get<base::Position>(e);
+    const Quat e_rot = ctx.get<base::Rotation>(e);
+    const Diag3x3 e_scale = ctx.get<base::Scale>(e);
+
+    const uint32_t num_prims = obj_mgr.rigidBodyPrimitiveCounts[e_obj_id.idx];
+    const uint32_t base_prim_offset = obj_mgr.rigidBodyPrimitiveOffsets[e_obj_id.idx];
+
+    const Vector3 axes[3] = { right, fwd, up };
+    for (uint32_t prim_offset = 0; prim_offset < num_prims; prim_offset++) {
+        const uint32_t prim_idx = base_prim_offset + prim_offset;
+        const CollisionPrimitive &prim = obj_mgr.collisionPrimitives[prim_idx];
+        if (prim.type != CollisionPrimitive::Type::Hull) continue;
+
+        const AABB txfmed_aabb = obj_mgr.primitiveAABBs[prim_idx].applyTRS(e_pos, e_rot, e_scale);
+        if (!txfmed_aabb.overlaps(aabb)) continue;
+
+        const Vector3 *vertices = prim.hull.halfEdgeMesh.vertices;
+        const CountT num_verts = (CountT)prim.hull.halfEdgeMesh.numVertices;
+        float min_hull_projs[3] = { FLT_MAX, FLT_MAX, FLT_MAX };
+        float max_hull_projs[3] = { -FLT_MAX, -FLT_MAX, -FLT_MAX };
+        for (CountT vert_idx = 0; vert_idx < num_verts; vert_idx++) {
+            const Vector3 v = e_rot.rotateVec(e_scale * vertices[vert_idx]) + e_pos;
+#pragma unroll
+            for (int i = 0; i < 3; i++) {
+                const float proj = dot(v, axes[i]);
+                if (proj < min_hull_projs[i]) min_hull_projs[i] = proj;
+                if (proj > max_hull_projs[i]) max_hull_projs[i] = proj;
+            }
+        }
+
+        bool axes_overlap = true;
+#pragma unroll
+        for (int i = 0; i < 3; i++) {
+            if (!(max_hull_projs[i] > aabb.pMin[i] && aabb.pMax[i] > min_hull_projs[i])) {
+                axes_overlap = false;
+            }
+        }
+        if (axes_overlap) return true;
+    }
+    return false;
+}
+
+// fn(e) for every entity whose leaf box overlaps aabb and that passes
+// checkEntityAABBOverlap, in the BVH's report order (reference: physics.inl:7-24).
+// One intended difference: a leaf whose entity was destroyed since the last
+// broadphase update is skipped (the reference reads whatever row the stale ID
+// points to).
+template <typename Fn>
+inline void findEntitiesWithinAABB(Context &ctx, math::AABB aabb, Fn &&fn)
+{
+    broadphase::BVH &bvh = ctx.singleton<broadphase::BVH>();
+    bvh.findIntersecting(aabb, [&](Entity e) {
+        if (!ctx.loc(e).valid()) return;
+        if (checkEntityAABBOverlap(ctx, aabb, e)) fn(e);
+    });
 }
 
 }

@@ -82,6 +82,11 @@ def _arena_objects():
     return arena_objects()
 
 
+def _triggers_objects():
+    from .objects import triggers_objects
+    return triggers_objects()
+
+
 def _room_render_cfg(cfg):
     from .render_assets import make_render_config
     return make_render_config(int(cfg.get("resolution", 64)), bool(cfg.get("rgbd", False)),
@@ -296,6 +301,61 @@ SIMS: Dict[str, SimDesc] = {
         defaults={"seed": 0},
         objects=_balls_objects,
         compile_flags=["-DBALLS_MANY=2"],
+    ),
+    # broadphase without the solver: standalone overlap rows (CandidateCollision), zone
+    # queries (findEntitiesWithinAABB / checkEntityAABBOverlap), a two-hull compound, a
+    # sphere, pickups destroyed and recreated (tests/test_overlap_queries.py)
+    "triggers": SimDesc(
+        name="triggers",
+        sources=[os.path.join(_ROOT, "triggers", "sim.cpp")],
+        num_exports=7,
+        num_taskgraphs=1,
+        inputs=[Slot(0, "action", "int32", (2, 2))],
+        outputs=[Slot(1, "pairs", "int32", (1 + 32 * 4,)), Slot(2, "zone", "int32", (8,)),
+                 Slot(3, "agent_pos", "float32", (2, 3)),
+                 Slot(4, "pickup_entity", "int32", (2,), dynamic=True),
+                 Slot(5, "pickup_pos", "float32", (3,), dynamic=True),
+                 Slot(6, "prop_entity", "int32", (7, 2))],
+        pack_config=lambda cfg: struct.pack("<Q", int(cfg.get("obj_mgr_ptr", 0))),
+        pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
+        oracle_extra=lambda cfg: [int(cfg.get("seed", 0))],
+        defaults={"seed": 0},
+        objects=_triggers_objects,
+    ),
+    # pressure plates after the XPBD step: findEntitiesWithinAABB on the refitted tree,
+    # checkEntityAABBOverlap goal zone, doors (static bodies) that follow their buttons,
+    # a sphere resting on a button, episode resets (tests/test_overlap_queries.py)
+    "buttons": SimDesc(
+        name="buttons",
+        sources=[os.path.join(_ROOT, "buttons", "sim.cpp")],
+        num_exports=8,
+        num_taskgraphs=1,
+        inputs=[Slot(0, "reset", "int32", (1,)), Slot(1, "action", "int32", (2, 3))],
+        outputs=[Slot(2, "button_state", "int32", (2, 4)), Slot(3, "door_pos", "float32", (2, 3)),
+                 Slot(4, "agent_pos", "float32", (2, 3)), Slot(5, "goal", "int32", (2,)),
+                 Slot(6, "body_pos", "float32", (3,), dynamic=True),
+                 Slot(7, "body_entity", "int32", (2,), dynamic=True)],
+        pack_config=lambda cfg: struct.pack("<QII", int(cfg.get("obj_mgr_ptr", 0)),
+                                            int(cfg["episode_len"]), 0),
+        pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
+        oracle_extra=lambda cfg: [int(cfg["episode_len"]), int(cfg.get("seed", 0))],
+        defaults={"episode_len": 100, "seed": 0},
+        objects=_balls_objects,
+    ),
+    # GPU only: the triggers graph plus setupPhysicsStepTasks, rejected at launch-graph build
+    "triggers_with_solver": SimDesc(
+        name="triggers_with_solver",
+        sources=[os.path.join(_ROOT, "triggers", "sim.cpp")],
+        num_exports=7,
+        num_taskgraphs=1,
+        inputs=[Slot(0, "action", "int32", (2, 2))],
+        outputs=[Slot(2, "zone", "int32", (8,))],
+        pack_config=lambda cfg: struct.pack("<Q", int(cfg.get("obj_mgr_ptr", 0))),
+        pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
+        oracle_extra=lambda cfg: [],
+        defaults={"seed": 0},
+        objects=_triggers_objects,
+        compile_flags=["-DTRIGGERS_WITH_SOLVER=1"],
     ),
     "gridworld": SimDesc(
         name="gridworld",

@@ -317,3 +317,84 @@ def room_objects_big_hull() -> Tuple[bytes, List[int]]:
         dict(mesh="plane", meta=static),
     ]
     return build_objects(specs)
+
+
+def build_compound_objects(specs, plane_extent: float = 1.0e5) -> Tuple[bytes, List[int]]:
+    """specs: one dict per object -- {"prims": [<half-edge mesh dict> | "plane" | ("sphere", r),
+    ...], "meta": bytes(52)}; an object may have several primitives (its body box is the union
+    of theirs).  Same blob layout as build_objects()."""
+    b = BlobBuilder()
+    mgr_off = b.add(b"\0" * 48)
+    prims = [p for sp in specs for p in sp["prims"]]
+    mesh_offs = {}
+    for m in prims:
+        if isinstance(m, dict) and id(m) not in mesh_offs:
+            mesh_offs[id(m)] = (b.add(m["half_edges"].tobytes()), b.add(m["face_base"].tobytes()),
+                                b.add(m["planes"].tobytes()), b.add(m["vertices"].tobytes()))
+    prim_size = 56
+    prims_off = b.add(b"\0" * (prim_size * len(prims)), align=16)
+    boxes = []
+    big = plane_extent
+    for i, m in enumerate(prims):
+        base = prims_off + i * prim_size
+        if isinstance(m, dict):
+            struct.pack_into("<I", b.buf, base, TYPE_HULL)
+            he, fb, pl, vt = mesh_offs[id(m)]
+            b.pointer_at(base + 8, he)
+            b.pointer_at(base + 16, fb)
+            b.pointer_at(base + 24, pl)
+            b.pointer_at(base + 32, vt)
+            struct.pack_into("<III", b.buf, base + 40, len(m["half_edges"]), len(m["planes"]),
+                             len(m["vertices"]))
+            boxes.append((m["vertices"].min(axis=0), m["vertices"].max(axis=0)))
+        elif m == "plane":
+            struct.pack_into("<I", b.buf, base, TYPE_PLANE)
+            boxes.append(([-big, -big, -big], [big, big, 0.0]))
+        else:
+            struct.pack_into("<I", b.buf, base, TYPE_SPHERE)
+            struct.pack_into("<f", b.buf, base + 8, float(m[1]))
+            boxes.append(([-m[1]] * 3, [m[1]] * 3))
+    prim_aabb_off = b.add(b"".join(struct.pack("<6f", *lo, *hi) for lo, hi in boxes))
+    body_boxes, offsets, counts, k = [], [], [], 0
+    for sp in specs:
+        n = len(sp["prims"])
+        lo = np.min([boxes[k + j][0] for j in range(n)], axis=0)
+        hi = np.max([boxes[k + j][1] for j in range(n)], axis=0)
+        body_boxes.append(struct.pack("<6f", *lo, *hi))
+        offsets.append(k)
+        counts.append(n)
+        k += n
+    body_aabb_off = b.add(b"".join(body_boxes))
+    offs_off = b.add(np.asarray(offsets, dtype=np.uint32).tobytes())
+    cnts_off = b.add(np.asarray(counts, dtype=np.uint32).tobytes())
+    meta_off = b.add(b"".join(sp["meta"] for sp in specs))
+    for i, target in enumerate([prims_off, prim_aabb_off, body_aabb_off, offs_off, cnts_off, meta_off]):
+        b.pointer_at(mgr_off + 8 * i, target)
+    return bytes(b.buf), b.relocs
+
+
+def shifted_box_half_edge_mesh(dx: float, dy: float, dz: float):
+    """The unit cube of box_half_edge_mesh() moved by (dx, dy, dz) in object space."""
+    box = box_half_edge_mesh()
+    v = box["vertices"] + np.array([dx, dy, dz], dtype=np.float32)
+    faces = [[0, 2, 3, 1], [4, 5, 7, 6], [0, 1, 5, 4], [2, 6, 7, 3], [0, 4, 6, 2], [1, 3, 7, 5]]
+    return build_half_edge_mesh(v, faces)
+
+
+def triggers_objects() -> Tuple[bytes, List[int]]:
+    """Objects of sims/triggers, in SimObject order: Agent, Pickup, Wall, Floor (plane),
+    Dumbbell (two unit boxes side by side along x, centred 0.6 from the origin: a compound
+    of two hull primitives), Ball (a sphere of radius 0.5).  Bodies are kinematic or static:
+    the fixture never runs the solver, so the mass data is nominal."""
+    box = box_half_edge_mesh()
+    static = _metadata(0.0, [0.0, 0.0, 0.0], 0.5, 0.5)
+    specs = [
+        dict(prims=[box], meta=static),                                            # Agent
+        dict(prims=[box], meta=static),                                            # Pickup
+        dict(prims=[box], meta=static),                                            # Wall
+        dict(prims=["plane"], meta=static),                                        # Floor
+        dict(prims=[shifted_box_half_edge_mesh(-0.6, 0.0, 0.0),
+                    shifted_box_half_edge_mesh(0.6, 0.0, 0.0)], meta=static),      # Dumbbell
+        dict(prims=[("sphere", 0.5)], meta=static),                                # Ball
+    ]
+    return build_compound_objects(specs)
