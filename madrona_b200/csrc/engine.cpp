@@ -366,7 +366,6 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
     // torch's `actions.copy_(...)` -- is ordered before the step graph
     MB2_CUDA(cudaStreamCreate(&ex->stream));
     ex->rowsPerWorldHint = envU64("MADRONA_B200_ROWS_PER_WORLD", 128);
-    g_pdl = envU64("MADRONA_B200_PDL", 0) != 0;
     ex->tableGrowth = envU64("MADRONA_B200_TABLE_GROWTH", 1) != 0;
 
     // ---- JIT the simulator
@@ -579,16 +578,7 @@ static bool enqueueNode(Executor *ex, uint32_t node_idx, cudaStream_t s)
         unsigned grid = (unsigned)std::max<uint64_t>(1, std::min(blocks, max_blocks));
         const NodeRecord *drec = &ex->dState->nodes[node_idx];
         void *args[1] = { (void *)&drec };
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(grid);
-        cfg.blockDim = dim3(256);
-        cfg.stream = s;
-        cudaLaunchAttribute attr;
-        attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr.val.programmaticStreamSerializationAllowed = g_pdl ? 1 : 0;
-        cfg.attrs = &attr;
-        cfg.numAttrs = 1;
-        MB2_CUDA(cudaLaunchKernelExC(&cfg, (const void *)ex->nodeKernels[r.kernelID], args));
+        MB2_CUDA(cudaLaunchKernel((const void *)ex->nodeKernels[r.kernelID], dim3(grid), dim3(256), args, 0, s));
         return true;
     }
     case NodeSortArchetype:

@@ -67,38 +67,6 @@ struct LaunchGraph {
 
 void setError(const std::string &msg);
 
-// Programmatic dependent launch (MADRONA_B200_PDL=1, default OFF): every engine
-// kernel starts with mb2::pdlSync() -- "let my dependents be scheduled now, then
-// wait for my prerequisites to have completed" -- and can be launched with the
-// programmatic stream-serialization attribute, so that the ~50 kernel -> kernel
-// edges of the captured step graph do not each pay a drain + launch latency.
-// Off by default: the step's kernels are multi-wave, so the parked blocks of the
-// next kernel would take resident slots from the current kernel's later waves.
-// Measured on an H100 80GB HBM3 at a 400 W power limit (bench.py --steps 200,
-// mean of 3 alternating runs, ms/step default vs PDL): room 1.512 vs 1.633, arena
-// 1.735 vs 2.044, room_render 11.79 vs 12.03, but gridworld 0.553 vs 0.548 and
-// sortcheck 0.923 vs 0.899.  Kept behind the switch; with it off pdlSync() is two
-// no-op instructions.
-extern bool g_pdl;
-
-#ifdef __CUDACC__
-template <typename... KArgs, typename... Args>
-inline void launchK(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args)
-{
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = s;
-    cudaLaunchAttribute attr;
-    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr.val.programmaticStreamSerializationAllowed = g_pdl ? 1 : 0;
-    cfg.attrs = &attr;
-    cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
-}
-#endif
-
 // ---- ahead-of-time engine kernels (kernels_core.cu / kernels_sort.cu) -----
 void launchClearTmp(Executor *ex, uint32_t archetype, cudaStream_t s);
 void launchResetTmpAlloc(Executor *ex, cudaStream_t s);

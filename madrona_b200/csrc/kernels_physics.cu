@@ -1616,7 +1616,6 @@ template <bool SPHERE_HULL>
 __global__ void __launch_bounds__(kNarrowThreads, SPHERE_HULL ? kNarrowMinBlocksSpheres : kNarrowMinBlocks)
 physNarrowphaseKernel(EngineState *Sp)
 {
-    pdlSync();
     EngineState &S = *Sp;
     const PhysicsState &P = *S.physics;
     fillColCache(S, P);
@@ -2314,7 +2313,6 @@ template <u32 OP>
 __global__ void __launch_bounds__(256, 1)
 physBodyKernel(EngineState *Sp)
 {
-    pdlSync();
     const EngineState &S = *Sp;
     const PhysicsState &P = *S.physics;
     if (blockIdx.y >= P.numBodyArchetypes) return;
@@ -2342,7 +2340,6 @@ physBodyKernel(EngineState *Sp)
 __global__ void __launch_bounds__(128)
 physRebuildKernel(EngineState *Sp)
 {
-    pdlSync();
     const EngineState &S = *Sp;
     const i32 w = blockIdx.x * blockDim.x + threadIdx.x;
     if (w >= (i32)S.numWorlds) return;
@@ -2356,7 +2353,6 @@ constexpr int kPhysWorldThreads = 32 * kPhysWarps;
 __global__ void __launch_bounds__(kPhysWorldThreads, 8)
 physFindCandidatesKernel(EngineState *Sp)
 {
-    pdlSync();
     EngineState &S = *Sp;
     const PhysicsState &P = *S.physics;
     fillColCache(S, P);
@@ -2385,7 +2381,6 @@ __device__ __forceinline__ bool solverWorld(const EngineState &S, i32 &w, bool &
 __global__ void __launch_bounds__(kPhysWorldThreads, 8)
 physSolvePositionsKernel(EngineState *Sp)
 {
-    pdlSync();
     EngineState &S = *Sp;
     const PhysicsState &P = *S.physics;
     fillColCache(S, P);
@@ -2403,7 +2398,6 @@ physSolvePositionsKernel(EngineState *Sp)
 __global__ void __launch_bounds__(kPhysWorldThreads, 8)
 physSolveVelocitiesKernel(EngineState *Sp)
 {
-    pdlSync();
     EngineState &S = *Sp;
     const PhysicsState &P = *S.physics;
     fillColCache(S, P);
@@ -2429,7 +2423,6 @@ constexpr int kEmitScanThreads = 1024;
 __global__ void __launch_bounds__(kEmitScanThreads)
 physEmitOverlapsScanKernel(EngineState *Sp, u32 archetype)
 {
-    pdlSync();
     EngineState &S = *Sp;
     const PhysicsState &P = *S.physics;
     TableDesc &t = S.tables[archetype];
@@ -2491,7 +2484,6 @@ struct OverlapRow {
 __global__ void __launch_bounds__(kPhysWorldThreads)
 physEmitOverlapsKernel(EngineState *Sp, u32 archetype, i32 col)
 {
-    pdlSync();
     const EngineState &S = *Sp;
     const PhysicsState &P = *S.physics;
     const i32 w = (i32)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
@@ -2668,8 +2660,8 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
             // tag 0 (post-integration) never rebuilds in the reference either; a
             // pending rebuild request then simply waits for the next tag-1 node,
             // and the un-refitted leaves are refitted by that rebuild
-            launchK(physBodyKernel<PhaseUpdateLeaves>, dim3(bgrid), dim3(256), 0, s, d);
-            if (rec.userTag == 1) launchK(physRebuildKernel, dim3((W + 127) / 128), dim3(128), 0, s, d);
+            physBodyKernel<PhaseUpdateLeaves><<<bgrid, 256, 0, s>>>(d);
+            if (rec.userTag == 1) physRebuildKernel<<<(W + 127) / 128, 128, 0, s>>>(d);
             break;
         case NodePhysFindCandidates:
             // joints are iterated per world by the solver: keep their table in
@@ -2678,33 +2670,33 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
             if (rec.userTag != 1) launchSortArchetype(ex, ph->hPhys.jointArchetype, 1, s);
             // the search appends the step's pairs to two empty lists
             cudaMemsetAsync(ph->hPhys.pairCounts, 0, 2 * sizeof(i32), s);
-            launchK(physFindCandidatesKernel, dim3(wgrid), dim3(wblock), 0, s, d);
+            physFindCandidatesKernel<<<wgrid, wblock, 0, s>>>(d);
             break;
         case NodePhysSubstepBegin:
-            launchK(physBodyKernel<PhaseIntegrate>, dim3(bgrid), dim3(256), 0, s, d);
+            physBodyKernel<PhaseIntegrate><<<bgrid, 256, 0, s>>>(d);
             break;
         case NodePhysNarrowphase:
             if (ph->narrowBlocks == 0) {
                 *err = "narrowphase occupancy query failed";
                 return false;
             }
-            if (ph->spheres) launchK(physNarrowphaseKernel<true>, dim3(ph->narrowBlocks), dim3(kNarrowThreads), 0, s, d);
-            else launchK(physNarrowphaseKernel<false>, dim3(ph->narrowBlocks), dim3(kNarrowThreads), 0, s, d);
+            if (ph->spheres) physNarrowphaseKernel<true><<<ph->narrowBlocks, kNarrowThreads, 0, s>>>(d);
+            else physNarrowphaseKernel<false><<<ph->narrowBlocks, kNarrowThreads, 0, s>>>(d);
             break;
         case NodePhysSolvePositions:
-            launchK(physSolvePositionsKernel, dim3(sgrid), dim3(wblock), 0, s, d);
+            physSolvePositionsKernel<<<sgrid, wblock, 0, s>>>(d);
             break;
         case NodePhysTGSVelocities:
-            launchK(physBodyKernel<PhaseTGSVelocities>, dim3(bgrid), dim3(256), 0, s, d);
+            physBodyKernel<PhaseTGSVelocities><<<bgrid, 256, 0, s>>>(d);
             break;
         case NodePhysTGSPositions:
-            launchK(physBodyKernel<PhaseTGSPositions>, dim3(bgrid), dim3(256), 0, s, d);
+            physBodyKernel<PhaseTGSPositions><<<bgrid, 256, 0, s>>>(d);
             break;
         case NodePhysSetVelocities:
-            launchK(physBodyKernel<PhaseSetVelocities>, dim3(bgrid), dim3(256), 0, s, d);
+            physBodyKernel<PhaseSetVelocities><<<bgrid, 256, 0, s>>>(d);
             break;
         case NodePhysSolveVelocities:
-            launchK(physSolveVelocitiesKernel, dim3(sgrid), dim3(wblock), 0, s, d);
+            physSolveVelocitiesKernel<<<sgrid, wblock, 0, s>>>(d);
             break;
         case NodePhysEmitOverlaps: {
             const EngineState &S = *ex->hState;
@@ -2714,8 +2706,8 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
                 *err = "standalone overlap node: the CandidateTemporary archetype lacks CandidateCollision";
                 return false;
             }
-            launchK(physEmitOverlapsScanKernel, dim3(1), dim3(kEmitScanThreads), 0, s, d, rec.archetype);
-            launchK(physEmitOverlapsKernel, dim3(wgrid), dim3(wblock), 0, s, d, rec.archetype, col);
+            physEmitOverlapsScanKernel<<<1, kEmitScanThreads, 0, s>>>(d, rec.archetype);
+            physEmitOverlapsKernel<<<wgrid, wblock, 0, s>>>(d, rec.archetype, col);
             break;
         }
         default:

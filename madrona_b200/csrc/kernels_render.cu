@@ -72,7 +72,6 @@ struct RenderCameraComp {     // == madrona::render::RenderCamera
 __global__ void __launch_bounds__(128)
 renderGatherInstancesKernel(EngineState *Sp)
 {
-    pdlSync();
     EngineState &S = *Sp;
     RenderState &R = *S.render;
     const int lane = threadIdx.x & 31;
@@ -142,7 +141,6 @@ __global__ void __launch_bounds__(256)
 renderLightUpdateKernel(EngineState *Sp, u32 archetype, i32 carrier_col, i32 pos_col, i32 dir_col, i32 type_col,
                         i32 shadow_col, i32 cutoff_col, i32 intensity_col, i32 active_col)
 {
-    pdlSync();
     EngineState &S = *Sp;
     const RenderState &R = *S.render;
     const TableDesc &t = S.tables[archetype];
@@ -171,7 +169,6 @@ renderLightUpdateKernel(EngineState *Sp, u32 archetype, i32 carrier_col, i32 pos
 __global__ void __launch_bounds__(256)
 renderGatherLightsKernel(EngineState *Sp)
 {
-    pdlSync();
     EngineState &S = *Sp;
     RenderState &R = *S.render;
     const TableDesc &t = S.tables[R.lightArchetype];
@@ -205,7 +202,6 @@ renderGatherLightsKernel(EngineState *Sp)
 __global__ void __launch_bounds__(256)
 renderGatherViewsKernel(EngineState *Sp)
 {
-    pdlSync();
     EngineState &S = *Sp;
     RenderState &R = *S.render;
     if (blockIdx.y >= R.numViewArchetypes) return;
@@ -295,7 +291,6 @@ __device__ __forceinline__ int commonPrefix(const unsigned long long *keys, int 
 __global__ void __launch_bounds__(32)
 renderBuildTLASKernel(EngineState *Sp)
 {
-    pdlSync();
     extern __shared__ __align__(16) unsigned char tlas_smem[];
     EngineState &S = *Sp;
     RenderState &R = *S.render;
@@ -884,7 +879,6 @@ template <bool FLAT, bool MATERIALS>
 __global__ void __launch_bounds__(256, kRaycastMinBlocks)
 renderRaycastKernel(EngineState *Sp)
 {
-    pdlSync();
     EngineState &S = *Sp;
     const RenderState &R = *S.render;
     const TableDesc &out_tbl = S.tables[R.outputArchetype];
@@ -1312,7 +1306,6 @@ void renderHostDestroy(Executor *ex)
 
 __global__ void renderResetCountsKernel(EngineState *Sp)
 {
-    pdlSync();
     Sp->render->totalNumInstances = 0;
 }
 
@@ -1323,25 +1316,25 @@ bool renderEnqueuePrepare(Executor *ex, cudaStream_t s, std::string *err)
     (void)err;
     const RenderState &R = rh->hRender;
     const unsigned W = ex->hState->numWorlds;
-    launchK(renderResetCountsKernel, dim3(1), dim3(1), 0, s, ex->dState);
-    launchK(renderGatherInstancesKernel, dim3((W * 32 + 127) / 128), dim3(128), 0, s, ex->dState);
+    renderResetCountsKernel<<<1, 1, 0, s>>>(ex->dState);
+    renderGatherInstancesKernel<<<(W * 32 + 127) / 128, 128, 0, s>>>(ex->dState);
     // lights: carriers refresh their light entities, the light table is brought into
     // world order (no-op when clean), then listed per world
     for (const LightCarrierArchetype &lc : lightCarriers(ex)) {
         const int cap = ex->hState->tables[lc.archetype].capacity;
-        launchK(renderLightUpdateKernel, dim3((unsigned)std::max(1, std::min((cap + 255) / 256, ex->numSMs * 2))),
-                dim3(256), 0, s, ex->dState, lc.archetype, lc.carrierCol, lc.posCol, lc.dirCol, lc.typeCol,
-                lc.shadowCol, lc.cutoffCol, lc.intensityCol, lc.activeCol);
+        renderLightUpdateKernel<<<(unsigned)std::max(1, std::min((cap + 255) / 256, ex->numSMs * 2)), 256, 0, s>>>(
+            ex->dState, lc.archetype, lc.carrierCol, lc.posCol, lc.dirCol, lc.typeCol,
+            lc.shadowCol, lc.cutoffCol, lc.intensityCol, lc.activeCol);
     }
     launchSortArchetype(ex, R.lightArchetype, 1, s);
-    launchK(renderGatherLightsKernel, dim3((W + 255) / 256), dim3(256), 0, s, ex->dState);
+    renderGatherLightsKernel<<<(W + 255) / 256, 256, 0, s>>>(ex->dState);
     int max_cap = 256;
     for (u32 i = 0; i < R.numViewArchetypes; i++) {
         max_cap = std::max(max_cap, ex->hState->tables[R.viewers[i].archetype].capacity);
     }
     dim3 grid((unsigned)std::min((max_cap + 255) / 256, ex->numSMs * 4), std::max(R.numViewArchetypes, 1u));
-    launchK(renderGatherViewsKernel, dim3(grid), dim3(256), 0, s, ex->dState);
-    launchK(renderBuildTLASKernel, dim3(W), dim3(32), rh->tlasSmem, s, ex->dState);
+    renderGatherViewsKernel<<<grid, 256, 0, s>>>(ex->dState);
+    renderBuildTLASKernel<<<W, 32, rh->tlasSmem, s>>>(ex->dState);
     return true;
 }
 
@@ -1389,11 +1382,11 @@ LaunchGraph *physicsBuildRenderGraph(Executor *ex, std::string *err)
     // 1024 worlds); 8 rounds of resident blocks keep the tail short
     const unsigned view_blocks = (unsigned)std::max(1, std::min(R.maxViews, ex->numSMs * kRaycastMinBlocks * 8));
     if (R.materials) {
-        launchK(renderRaycastKernel<true, true>, dim3(1, view_blocks), dim3(256), 0, ex->stream, ex->dState);
-        launchK(renderRaycastKernel<false, true>, dim3(1, view_blocks), dim3(256), 0, ex->stream, ex->dState);
+        renderRaycastKernel<true, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+        renderRaycastKernel<false, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
     } else {
-        launchK(renderRaycastKernel<true, false>, dim3(1, view_blocks), dim3(256), 0, ex->stream, ex->dState);
-        launchK(renderRaycastKernel<false, false>, dim3(1, view_blocks), dim3(256), 0, ex->stream, ex->dState);
+        renderRaycastKernel<true, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+        renderRaycastKernel<false, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
     }
     launchStatusCopy(ex, ex->stream);
     cudaError_t e = cudaStreamEndCapture(ex->stream, &g->graph);

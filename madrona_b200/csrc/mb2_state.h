@@ -218,13 +218,4 @@ enum ErrorFlags : u32 {
     ErrRenderAsset = 1u << 7,          // a material names a texture the render config does not have
 };
 
-#ifdef __CUDACC__
-// First statement of every engine / simulator kernel (see engine.hpp launchK).
-__device__ __forceinline__ void pdlSync()
-{
-    asm volatile("griddepcontrol.launch_dependents;");
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-}
-#endif
-
 }
