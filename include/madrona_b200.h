@@ -214,11 +214,14 @@ int64_t mb2_get_exported_row_bytes(const mb2_executor *exec, int64_t slot);
 void *mb2_render_debug_hits(mb2_executor *exec);
 
 /* Test hook: the ray caster's per-world structures of the last render-prepare.
- * which = 1: QBVHNode [worlds][max_instances] (TLAS, node 0 = root), 2: int32
- * TLAS node counts [worlds], 3: instances [worlds][max_instances] (76-byte
- * records: position, rotation, scale, matID, objectID, colour, world box),
- * 4: int32 instance counts [worlds].  Device pointers; NULL without a renderer. */
-void *mb2_render_debug_buffer(mb2_executor *exec, int which, int64_t *max_instances_per_world);
+ * The layouts are compact: world w's instances and TLAS nodes start at entry
+ * offsets[w] of one list (offsets = exclusive scan of the instance counts).
+ * which = 1: QBVHNode list (world w's tree at offsets[w], node 0 = root), 2: int32
+ * TLAS node counts [worlds], 3: instance list (76-byte records: position,
+ * rotation, scale, matID, objectID, colour, world box), 4: int32 instance counts
+ * [worlds], 5: int32 instance offsets [worlds].  *stride is set to 0 (there is
+ * no per-world stride).  Device pointers; NULL without a renderer. */
+void *mb2_render_debug_buffer(mb2_executor *exec, int which, int64_t *stride);
 
 /* Kernel nodes inside a built launch graph (== launches per run). */
 int64_t mb2_launch_graph_num_kernels(const mb2_launch_graph *graph);

@@ -71,6 +71,9 @@ static std::string describeErrors(uint32_t flags, uint32_t archetype)
     if (flags & ErrPhysicsOverflow) s += "physics buffer overflow ";
     if (flags & ErrRenderAsset) s += "render asset error (a material's textureIdx is not below "
         "materialData.numTextureBuffers; those pixels were shaded untextured) ";
+    if (flags & ErrRenderCapacity) s += "render instance list overflow ";
+    if (flags & ErrRenderTLASDepth) s += "render TLAS too deep for the ray caster's traversal stack (a world's "
+        "renderables are too tightly clustered) ";
     return s;
 }
 
@@ -262,6 +265,8 @@ bool growTable(Executor *ex, uint32_t a, int64_t new_cap, std::string *err)
     t.capacity = (int32_t)new_cap;
     cudaMemcpy(&ex->dState->tables[a].capacity, &t.capacity, sizeof(int32_t), cudaMemcpyHostToDevice);
     cudaMemcpy(&ex->dState->entityCapacity, &S.entityCapacity, sizeof(int32_t), cudaMemcpyHostToDevice);
+    // the ray caster's instance list has a row for every renderable row
+    if (!renderEnsureCapacity(ex, err)) return false;
     ex->growthEvents++;
     if (getenv("MADRONA_B200_VERBOSE")) {
         fprintf(stderr, "[madrona_b200] archetype %u grown to %ld rows\n", a, (long)new_cap);
@@ -935,6 +940,7 @@ static int64_t profileNodes(Executor *ex, const uint32_t *ids, uint32_t n, uint3
             int64_t rows;
             physicsNodeBytes(ex, r, &kn, &rows);
         }
+        if (r.kind == NodeRenderPrepare) kn = "render_prepare";
         std::string name = kn;
         if (r.kind == NodeUserParallelFor && r.kernelID < ex->jit.nodeKernels.size()) {
             // keep the mangled system name readable: take the part after "_Z" of the NTTP
@@ -1167,12 +1173,11 @@ void *mb2_render_debug_hits(mb2_executor *exec)
     return exec ? renderDebugHitBuffer((Executor *)exec) : nullptr;
 }
 
-void *mb2_render_debug_buffer(mb2_executor *exec, int which, int64_t *max_instances_per_world)
+void *mb2_render_debug_buffer(mb2_executor *exec, int which, int64_t *stride)
 {
-    int64_t stride = 0;
-    void *p = exec ? renderDebugBuffer((Executor *)exec, which, &stride) : nullptr;
-    if (max_instances_per_world) *max_instances_per_world = stride;
-    return p;
+    // the layouts are compact (world w at instance offset w): no per-world stride
+    if (stride) *stride = 0;
+    return exec ? renderDebugBuffer((Executor *)exec, which) : nullptr;
 }
 
 int64_t mb2_launch_graph_num_branches(const mb2_launch_graph *graph)

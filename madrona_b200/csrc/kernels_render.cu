@@ -6,15 +6,21 @@
 // three archetype sorts / bvhBuildFast / bvhConstructAABBs / bvhWidenTree /
 // exportCountsGPU: src/render/ecs_system.cpp:100-348, 486-597 and
 // src/mw/device/bvh.cpp:731-1217):
+//   renderCountInstancesKernel   visible renderables per world
+//   renderScanInstancesKernel    world offsets into the compact instance list, list of the
+//                                worlds above kWarpTLASInstances
 //   renderGatherInstancesKernel  every world's renderable instances -> InstanceData +
-//                                world box (mesh root box under TRS)
+//                                world box (mesh root box under TRS), at the world's offset
 //   renderLightKernels           carriers refresh their LightDesc, lights gathered per world
 //   renderGatherViewsKernel      PerspectiveCameraData per view
-//   renderBuildTLASKernel        ONE WARP PER WORLD, all in shared memory: 30-bit Morton
-//                                codes of the box centres inside the world's bounds, rank
-//                                sort, Karras' parallel LBVH, bottom-up boxes, collapse to
-//                                4-wide nodes, quantise -> QBVHNode[] (the reference's
-//                                traversal format)
+//   renderBuildTLASKernel        worlds of <= kWarpTLASInstances: ONE WARP PER WORLD, all in
+//                                shared memory: 30-bit Morton codes of the box centres inside
+//                                the world's bounds, rank sort, Karras' parallel LBVH,
+//                                bottom-up boxes, collapse to 4-wide nodes, quantise ->
+//                                QBVHNode[] (the reference's traversal format)
+//   renderBuildLargeTLASKernel   larger worlds: the same tree, one block per world taken by
+//                                ticket, scratch in global memory, bitonic key sort staged
+//                                through shared memory in kSortChunk tiles
 // Render graph: renderRaycastKernel, one thread per pixel, one block per view
 // (8 x 4 pixel tiles per warp): TLAS -> instance -> object-space ray -> BLAS
 // (reference-format MeshBVH: quantised 4-wide nodes over de-indexed triangles)
@@ -59,7 +65,33 @@ struct RenderHost {
     RenderState hRender;
     bool active = false;
     size_t tlasSmem = 0;
+    // instance list, TLAS nodes, large-world key / node scratch: one entry per renderable row
+    VMRange instanceRange, nodeRange, keyRange, buildRange;
 };
+
+// scratch entry of renderBuildLargeTLASKernel, one per instance of the world
+struct TLASBuildNode {
+    float box[6];           // binary internal node: min xyz, max xyz
+    i32 left, right;        // children: >= 0 internal, < 0: ~leaf (sorted position)
+    i32 parent;             // of internal node i (-1: root)
+    i32 leafParent;         // of the leaf at sorted position i
+    i32 arrivals;           // bottom-up arrival counter
+    i32 wideBin;            // binary node of wide node i
+    i32 wideDepth;          // level of wide node i (root: 1)
+};
+
+// worlds up to this size build their TLAS in one warp's shared memory (renderBuildTLASKernel)
+constexpr int kWarpTLASInstances = 128;
+constexpr int kLargeTLASThreads = 512;
+constexpr int kSortChunk = 4096;        // keys sorted per shared-memory pass (32 KiB)
+
+// Visible renderable of world w at `row`: the row belongs to w and its Renderable names an entity
+__device__ __forceinline__ bool renderableVisible(const TableDesc &t, const RenderArchetype &ra, i32 row, i32 w)
+{
+    if (((const i32 *)t.columns[1])[row] != w) return false;
+    const u64 marker = ((const u64 *)t.columns[ra.cols[RCRenderable]])[row];
+    return (i32)(u32)(marker >> 32) != -1;     // Renderable{Entity::none()} => hidden
+}
 
 struct RenderCameraComp {     // == madrona::render::RenderCamera
     u32 outGen; i32 outID;
@@ -69,6 +101,106 @@ struct RenderCameraComp {     // == madrona::render::RenderCamera
 };
 
 // ---- render-prepare: instances ---------------------------------------------------------
+// count, scan, write: world w's instances land at instanceOffsets[w] in gather order
+// (renderable archetypes ascending, then row order; instance k = k-th visible renderable)
+__global__ void __launch_bounds__(128)
+renderCountInstancesKernel(EngineState *Sp)
+{
+    EngineState &S = *Sp;
+    RenderState &R = *S.render;
+    const int lane = threadIdx.x & 31;
+    const i32 w = (i32)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    if (w >= (i32)S.numWorlds) return;
+    i32 running = 0;
+    for (u32 ai = 0; ai < R.numRenderArchetypes; ai++) {
+        const RenderArchetype &ra = R.renderables[ai];
+        const TableDesc &t = S.tables[ra.archetype];
+        const i32 first = t.worldOffsets[w];
+        const i32 count = t.worldCounts[w];
+        for (i32 base = 0; base < count; base += 32) {
+            const bool valid = base + lane < count && renderableVisible(t, ra, first + base + lane, w);
+            running += __popc(__ballot_sync(0xffffffffu, valid));
+        }
+    }
+    if (lane == 0) R.instanceCounts[w] = running;
+}
+
+// one block: exclusive scan of the counts -> offsets, and the worlds the large builder takes.
+// Each thread owns kScanWorlds consecutive worlds (independent loads), so 16384 worlds take
+// one pass of the block.
+constexpr int kScanWorlds = 16;
+
+__global__ void __launch_bounds__(1024)
+renderScanInstancesKernel(EngineState *Sp)
+{
+    EngineState &S = *Sp;
+    RenderState &R = *S.render;
+    __shared__ i32 s_warp[2][32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const i32 W = (i32)S.numWorlds;
+    long long carry = 0;
+    i32 large_carry = 0;
+    for (i32 base = 0; base < W; base += 1024 * kScanWorlds) {
+        const i32 first = base + (i32)threadIdx.x * kScanWorlds;
+        i32 counts[kScanWorlds];
+        i32 n = 0, large = 0;
+#pragma unroll
+        for (int k = 0; k < kScanWorlds; k++) {
+            counts[k] = first + k < W ? R.instanceCounts[first + k] : 0;
+            n += counts[k];
+            large += counts[k] > kWarpTLASInstances ? 1 : 0;
+        }
+        i32 a = n, b = large;
+        for (int o = 1; o < 32; o <<= 1) {
+            const i32 ua = __shfl_up_sync(0xffffffffu, a, o), ub = __shfl_up_sync(0xffffffffu, b, o);
+            if (lane >= o) {
+                a += ua;
+                b += ub;
+            }
+        }
+        if (lane == 31) {
+            s_warp[0][warp] = a;
+            s_warp[1][warp] = b;
+        }
+        __syncthreads();
+        if (warp == 0) {
+            i32 x = s_warp[0][lane], y = s_warp[1][lane];
+            for (int o = 1; o < 32; o <<= 1) {
+                const i32 ux = __shfl_up_sync(0xffffffffu, x, o), uy = __shfl_up_sync(0xffffffffu, y, o);
+                if (lane >= o) {
+                    x += ux;
+                    y += uy;
+                }
+            }
+            s_warp[0][lane] = x;
+            s_warp[1][lane] = y;
+        }
+        __syncthreads();
+        long long off = carry + (warp > 0 ? s_warp[0][warp - 1] : 0) + a - n;
+        i32 slot = large_carry + (warp > 0 ? s_warp[1][warp - 1] : 0) + b - large;
+#pragma unroll
+        for (int k = 0; k < kScanWorlds; k++) {
+            const i32 w = first + k;
+            if (w < W) {
+                R.instanceOffsets[w] = (i32)min(off, (long long)R.instanceCapacity);
+                if (counts[k] > kWarpTLASInstances) R.largeWorlds[slot++] = w;
+            }
+            off += counts[k];
+        }
+        carry += s_warp[0][31];
+        large_carry += s_warp[1][31];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        // exportCountsGPU (ecs_system.cpp:317-348)
+        R.totalNumInstances = (u32)min(carry, (long long)R.instanceCapacity);
+        R.numLargeWorlds = (u32)large_carry;
+        R.largeTicket = 0;
+        // the list has a row per renderable row, so this only trips on a broken table
+        if (carry > R.instanceCapacity) atomicOr(&S.errorFlags, (u32)ErrRenderCapacity);
+    }
+}
+
 __global__ void __launch_bounds__(128)
 renderGatherInstancesKernel(EngineState *Sp)
 {
@@ -78,7 +210,9 @@ renderGatherInstancesKernel(EngineState *Sp)
     const i32 w = (i32)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
     if (w >= (i32)S.numWorlds) return;
 
-    RenderInstance *out = R.instances + (size_t)w * R.maxInstancesPerWorld;
+    const i32 offset = R.instanceOffsets[w];
+    RenderInstance *out = R.instances + offset;
+    const i32 room = R.instanceCapacity - offset;
     i32 running = 0;
     for (u32 ai = 0; ai < R.numRenderArchetypes; ai++) {
         const RenderArchetype &ra = R.renderables[ai];
@@ -87,15 +221,11 @@ renderGatherInstancesKernel(EngineState *Sp)
         const i32 count = t.worldCounts[w];
         for (i32 base = 0; base < count; base += 32) {
             const i32 row = first + base + lane;
-            bool valid = base + lane < count && ((const i32 *)t.columns[1])[row] == w;
-            if (valid) {
-                const u64 marker = ((const u64 *)t.columns[ra.cols[RCRenderable]])[row];
-                valid = (i32)(u32)(marker >> 32) != -1;     // Renderable{Entity::none()} => hidden
-            }
+            const bool valid = base + lane < count && renderableVisible(t, ra, row, w);
             const u32 keep = __ballot_sync(0xffffffffu, valid);
             if (valid) {
                 const i32 at = running + __popc(keep & ((1u << lane) - 1u));
-                if (at < R.maxInstancesPerWorld) {
+                if (at < room) {
                     RenderInstance inst;
                     const Vector3 p = ((const Vector3 *)t.columns[ra.cols[RCPosition]])[row];
                     const Quat q = ((const Quat *)t.columns[ra.cols[RCRotation]])[row];
@@ -124,14 +254,8 @@ renderGatherInstancesKernel(EngineState *Sp)
             running += __popc(keep);
         }
     }
-    if (lane == 0) {
-        if (running > R.maxInstancesPerWorld) {
-            atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
-            running = R.maxInstancesPerWorld;
-        }
-        R.instanceCounts[w] = running;
-        atomicAdd(&R.totalNumInstances, (u32)running);
-    }
+    // an overflowing world (ErrRenderCapacity) keeps what fits
+    if (lane == 0 && running > room) R.instanceCounts[w] = max(room, 0);
 }
 
 // ---- render-prepare: lights -------------------------------------------------------------
@@ -288,6 +412,29 @@ __device__ __forceinline__ int commonPrefix(const unsigned long long *keys, int 
     return __clzll((long long)(keys[i] ^ keys[j]));     // keys are unique (index in the low word)
 }
 
+// Surface-area measure the 4-wide collapse ranks inner children by: dx*dy + dy*dz + dz*dx
+// with its fmas spelled out, so both builders (and tests/tlas_model.py) round it alike.
+__device__ __forceinline__ float wideChildArea(const float *b)
+{
+    const float dx = b[3] - b[0], dy = b[4] - b[1], dz = b[5] - b[2];
+    return __fmaf_rn(dx, dz, __fmaf_rn(dx, dy, __fmul_rn(dy, dz)));
+}
+
+// Traversal budget (traceWorld): kTraceStack entries per ray, shared by the TLAS and the
+// BLAS.  A TLAS of wide depth D holds at most 3 D entries when a BLAS walk starts, so trees
+// deeper than kMaxTLASDepth are refused (ErrRenderTLASDepth) rather than walked with nodes
+// dropped; the BLAS keeps at least kBLASStackReserve entries.
+constexpr int kTraceStack = 48;
+constexpr int kBLASStackReserve = 12;
+constexpr int kMaxTLASDepth = (kTraceStack - kBLASStackReserve) / 3;
+constexpr int kFlatInstances = 64;      // worlds up to this size are traced without their TLAS
+
+__device__ __forceinline__ void recordTLASDepth(EngineState &S, RenderState &R, i32 w, i32 n, int depth)
+{
+    R.tlasDepths[w] = depth;
+    if (depth > kMaxTLASDepth && n > kFlatInstances) atomicOr(&S.errorFlags, (u32)ErrRenderTLASDepth);
+}
+
 __global__ void __launch_bounds__(32)
 renderBuildTLASKernel(EngineState *Sp)
 {
@@ -297,13 +444,18 @@ renderBuildTLASKernel(EngineState *Sp)
     const int lane = threadIdx.x;
     const i32 w = (i32)blockIdx.x;
     const i32 n = R.instanceCounts[w];
-    const RenderInstance *inst = R.instances + (size_t)w * R.maxInstancesPerWorld;
-    QBVHNode *out = R.tlasNodes + (size_t)w * R.maxInstancesPerWorld;
+    if (n > kWarpTLASInstances) return;         // renderBuildLargeTLASKernel's
+    const i32 offset = R.instanceOffsets[w];
+    const RenderInstance *inst = R.instances + offset;
+    QBVHNode *out = R.tlasNodes + offset;
     if (n <= 0) {
-        if (lane == 0) R.tlasNodeCounts[w] = 0;
+        if (lane == 0) {
+            R.tlasNodeCounts[w] = 0;
+            R.tlasDepths[w] = 0;
+        }
         return;
     }
-    const int cap = R.maxInstancesPerWorld;
+    const int cap = kWarpTLASInstances;
     TLASScratch sc;
     {
         unsigned char *p = tlas_smem;
@@ -390,6 +542,7 @@ renderBuildTLASKernel(EngineState *Sp)
             node.triSize[0] = 0;
             out[0] = node;
             R.tlasNodeCounts[w] = 1;
+            recordTLASDepth(S, R, w, n, 1);
         }
         return;
     }
@@ -442,12 +595,14 @@ renderBuildTLASKernel(EngineState *Sp)
     }
     __syncwarp();
 
-    // 5. collapse to 4-wide nodes, breadth first; flags[0] now counts wide nodes
+    // 5. collapse to 4-wide nodes, breadth first; flags[0] now counts wide nodes, flags[k]
+    // (k >= 1, free after step 4) holds wide node k's level
     if (lane == 0) {
         sc.wideBin[0] = 0;
         sc.flags[0] = 1;
     }
     __syncwarp();
+    int depth = 1;
     // waves: nodes [done, count) exist and are not written yet; writing them appends
     // their inner children behind `count`
     for (int done = 0;;) {
@@ -457,6 +612,7 @@ renderBuildTLASKernel(EngineState *Sp)
         __syncwarp();
         if (k < count_now) {
             const int bin = sc.wideBin[k];
+            const int level = k == 0 ? 1 : sc.flags[k];
             int kids[kBVHWidth];
             int nk = 2;
             kids[0] = sc.left[bin];
@@ -466,9 +622,7 @@ renderBuildTLASKernel(EngineState *Sp)
                 float best = -1.f;
                 for (int c = 0; c < nk; c++) {
                     if (kids[c] < 0) continue;
-                    const float *b = sc.nodeBox + kids[c] * 6;
-                    const float dx = b[3] - b[0], dy = b[4] - b[1], dz = b[5] - b[2];
-                    const float area = dx * dy + dy * dz + dz * dx;
+                    const float area = wideChildArea(sc.nodeBox + kids[c] * 6);
                     if (area > best) {
                         best = area;
                         pick = c;
@@ -496,6 +650,8 @@ renderBuildTLASKernel(EngineState *Sp)
                 } else {
                     const int id = atomicAdd(&sc.flags[0], 1);
                     sc.wideBin[id] = (short)kids[c];
+                    sc.flags[id] = level + 1;
+                    depth = max(depth, level + 1);
                     node.childrenIdx[c] = (u32)id;
                 }
             }
@@ -504,7 +660,274 @@ renderBuildTLASKernel(EngineState *Sp)
         __syncwarp();
         done = min(done + 32, count_now);
     }
-    if (lane == 0) R.tlasNodeCounts[w] = sc.flags[0];
+    depth = __reduce_max_sync(0xffffffffu, depth);
+    if (lane == 0) {
+        R.tlasNodeCounts[w] = sc.flags[0];
+        recordTLASDepth(S, R, w, n, depth);
+    }
+}
+
+// ---- render-prepare: TLAS of worlds above kWarpTLASInstances --------------------------------
+// One step of an ascending bitonic sorting network over keys [0, npad) (npad a power of
+// two); keys past n act as +inf and never move.  flip: first step of merging sorted runs of
+// j into runs of 2 j (partner mirrored in the run), else a half-cleaner (partner i + j).
+// Every comparator puts the smaller key first, which is what lets the tail stay virtual.
+__device__ __forceinline__ void bitonicStep(unsigned long long *k, int n, int npad, int j, bool flip)
+{
+    for (int t = threadIdx.x; t < (npad >> 1); t += blockDim.x) {
+        const int low = t & (j - 1);
+        const int i = ((t - low) << 1) + low;
+        const int p = flip ? i + 2 * (j - low) - 1 : i + j;
+        if (p < n) {
+            const unsigned long long a = k[i], b = k[p];
+            if (a > b) {
+                k[i] = b;
+                k[p] = a;
+            }
+        }
+    }
+}
+
+// Block-wide sort of n unique keys in global memory: every kSortChunk tile sorted in shared
+// memory, then each merge level's strides >= kSortChunk in global memory and the rest per
+// tile in shared memory.
+__device__ void blockSortKeys(unsigned long long *g, int n, unsigned long long *s)
+{
+    int npad = 1;
+    while (npad < n) npad <<= 1;
+    const int C = min(npad, kSortChunk);
+    // whole: sort the tile; else: the current level's half-cleaners with strides below C
+    auto tile = [&](int c0, bool whole) {
+        const int m = min(C, n - c0);
+        for (int i = threadIdx.x; i < C; i += blockDim.x) s[i] = i < m ? g[c0 + i] : ~0ull;
+        __syncthreads();
+        auto halfCleaners = [&](int from) {
+            for (int j = from; j >= 1; j >>= 1) {
+                bitonicStep(s, C, C, j, false);
+                __syncthreads();
+            }
+        };
+        if (whole) {
+            for (int size = 2; size <= C; size <<= 1) {
+                bitonicStep(s, C, C, size >> 1, true);
+                __syncthreads();
+                halfCleaners(size >> 2);
+            }
+        } else {
+            halfCleaners(C >> 1);
+        }
+        for (int i = threadIdx.x; i < m; i += blockDim.x) g[c0 + i] = s[i];
+        __syncthreads();
+    };
+    for (int c0 = 0; c0 < n; c0 += C) tile(c0, true);
+    for (int size = 2 * C; size <= npad; size <<= 1) {
+        bitonicStep(g, n, npad, size >> 1, true);
+        __syncthreads();
+        for (int j = size >> 2; j >= C; j >>= 1) {
+            bitonicStep(g, n, npad, j, false);
+            __syncthreads();
+        }
+        for (int c0 = 0; c0 < n; c0 += C) tile(c0, false);
+    }
+}
+
+// One block per world, worlds taken by ticket from the scan's list (a step without large
+// worlds costs one launch of blocks that find the list empty).  Same rules as the warp
+// builder, so the same tree: bounds of the box centres, Morton key << 32 | gather index,
+// Karras' split over the sorted keys, bottom-up boxes with arrival counters, 4-wide collapse
+// expanding the inner child of largest area (first maximum wins), quantizeNode.
+__global__ void __launch_bounds__(kLargeTLASThreads)
+renderBuildLargeTLASKernel(EngineState *Sp)
+{
+    __shared__ unsigned long long s_keys[kSortChunk];
+    __shared__ float s_bounds[6][kLargeTLASThreads / 32];
+    __shared__ i32 s_world, s_count, s_depth;
+    EngineState &S = *Sp;
+    RenderState &R = *S.render;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (;;) {
+        if (threadIdx.x == 0) {
+            const u32 t = atomicAdd(&R.largeTicket, 1u);
+            s_world = t < R.numLargeWorlds ? R.largeWorlds[t] : -1;
+        }
+        __syncthreads();
+        const i32 w = s_world;
+        if (w < 0) return;
+        const i32 n = R.instanceCounts[w];
+        const i32 offset = R.instanceOffsets[w];
+        const RenderInstance *inst = R.instances + offset;
+        unsigned long long *keys = R.tlasKeys + offset;
+        TLASBuildNode *bn = R.tlasBuild + offset;
+        QBVHNode *out = R.tlasNodes + offset;
+
+        // 1. bounds of the box centres, Morton keys
+        float lo[3] = { FLT_MAX, FLT_MAX, FLT_MAX }, hi[3] = { -FLT_MAX, -FLT_MAX, -FLT_MAX };
+        for (int i = threadIdx.x; i < n; i += blockDim.x) {
+            for (int a = 0; a < 3; a++) {
+                const float c = 0.5f * (inst[i].aabbMin[a] + inst[i].aabbMax[a]);
+                lo[a] = fminf(lo[a], c);
+                hi[a] = fmaxf(hi[a], c);
+            }
+        }
+        for (int o = 16; o >= 1; o >>= 1) {
+            for (int a = 0; a < 3; a++) {
+                lo[a] = fminf(lo[a], __shfl_xor_sync(0xffffffffu, lo[a], o));
+                hi[a] = fmaxf(hi[a], __shfl_xor_sync(0xffffffffu, hi[a], o));
+            }
+        }
+        if (lane == 0) {
+            for (int a = 0; a < 3; a++) {
+                s_bounds[a][warp] = lo[a];
+                s_bounds[3 + a][warp] = hi[a];
+            }
+        }
+        __syncthreads();
+        for (int a = 0; a < 3; a++) {
+            lo[a] = s_bounds[a][0];
+            hi[a] = s_bounds[3 + a][0];
+            for (int k = 1; k < kLargeTLASThreads / 32; k++) {
+                lo[a] = fminf(lo[a], s_bounds[a][k]);
+                hi[a] = fmaxf(hi[a], s_bounds[3 + a][k]);
+            }
+        }
+        for (int i = threadIdx.x; i < n; i += blockDim.x) {
+            u32 code = 0;
+            for (int a = 0; a < 3; a++) {
+                const float c = 0.5f * (inst[i].aabbMin[a] + inst[i].aabbMax[a]);
+                const float ext = hi[a] - lo[a];
+                float u = ext > 0.f ? (c - lo[a]) / ext : 0.f;
+                u = fminf(fmaxf(u * 1024.f, 0.f), 1023.f);
+                code |= expandBits10((u32)u) << a;
+            }
+            keys[i] = ((unsigned long long)code << 32) | (u32)i;
+        }
+        __syncthreads();
+
+        // 2. sort; the low word of a sorted key is the instance's gather index
+        blockSortKeys(keys, n, s_keys);
+
+        // 3. Karras 2012 over the sorted keys
+        for (int i = threadIdx.x; i < n - 1; i += blockDim.x) {
+            const int d = commonPrefix(keys, n, i, i + 1) - commonPrefix(keys, n, i, i - 1) >= 0 ? 1 : -1;
+            const int delta_min = commonPrefix(keys, n, i, i - d);
+            int lmax = 2;
+            while (commonPrefix(keys, n, i, i + lmax * d) > delta_min) lmax <<= 1;
+            int l = 0;
+            for (int t = lmax >> 1; t >= 1; t >>= 1) {
+                if (commonPrefix(keys, n, i, i + (l + t) * d) > delta_min) l += t;
+            }
+            const int j = i + l * d;
+            const int delta_node = commonPrefix(keys, n, i, j);
+            int s = 0;
+            for (int t = (l + 1) >> 1; ; t = (t + 1) >> 1) {
+                if (commonPrefix(keys, n, i, i + (s + t) * d) > delta_node) s += t;
+                if (t == 1) break;
+            }
+            const int gamma = i + s * d + min(d, 0);
+            const int first = min(i, j), last = max(i, j);
+            const int lc = first == gamma ? ~gamma : gamma;
+            const int rc = last == gamma + 1 ? ~(gamma + 1) : gamma + 1;
+            bn[i].left = lc;
+            bn[i].right = rc;
+            bn[i].arrivals = 0;
+            if (lc >= 0) bn[lc].parent = i; else bn[~lc].leafParent = i;
+            if (rc >= 0) bn[rc].parent = i; else bn[~rc].leafParent = i;
+        }
+        if (threadIdx.x == 0) bn[0].parent = -1;
+        __syncthreads();
+
+        // 4. boxes, bottom-up: the second thread to reach a node owns it (boxes other threads
+        // wrote are read from L2)
+        auto leafBox = [&](int pos, int a) {
+            const RenderInstance &ri = inst[(u32)keys[pos]];
+            return a < 3 ? ri.aabbMin[a] : ri.aabbMax[a - 3];
+        };
+        for (int leaf = threadIdx.x; leaf < n; leaf += blockDim.x) {
+            int node = bn[leaf].leafParent;
+            while (node >= 0) {
+                __threadfence();
+                if (atomicAdd(&bn[node].arrivals, 1) == 0) break;
+                const int lc = __ldcg(&bn[node].left), rc = __ldcg(&bn[node].right);
+                float b[6];
+                for (int a = 0; a < 6; a++) {
+                    const float lv = lc >= 0 ? __ldcg(&bn[lc].box[a]) : leafBox(~lc, a);
+                    const float rv = rc >= 0 ? __ldcg(&bn[rc].box[a]) : leafBox(~rc, a);
+                    b[a] = a < 3 ? fminf(lv, rv) : fmaxf(lv, rv);
+                }
+                for (int a = 0; a < 6; a++) bn[node].box[a] = b[a];
+                node = __ldcg(&bn[node].parent);
+            }
+        }
+        __syncthreads();
+
+        // 5. collapse to 4-wide nodes, breadth first in waves: nodes [done, count) exist and
+        // are not written yet; writing them appends their inner children behind `count`
+        if (threadIdx.x == 0) {
+            bn[0].wideBin = 0;
+            bn[0].wideDepth = 1;
+            s_count = 1;
+            s_depth = 1;
+        }
+        __syncthreads();
+        for (int done = 0;;) {
+            const int count_now = s_count;
+            __syncthreads();
+            if (done >= count_now) break;
+            for (int k = done + threadIdx.x; k < count_now; k += blockDim.x) {
+                const int bin = bn[k].wideBin;
+                const int level = bn[k].wideDepth;
+                int kids[kBVHWidth];
+                int nk = 2;
+                kids[0] = bn[bin].left;
+                kids[1] = bn[bin].right;
+                while (nk < kBVHWidth) {
+                    int pick = -1;
+                    float best = -1.f;
+                    for (int c = 0; c < nk; c++) {
+                        if (kids[c] < 0) continue;
+                        const float area = wideChildArea(bn[kids[c]].box);
+                        if (area > best) {
+                            best = area;
+                            pick = c;
+                        }
+                    }
+                    if (pick < 0) break;
+                    const int inner = kids[pick];
+                    kids[pick] = bn[inner].left;
+                    kids[nk++] = bn[inner].right;
+                }
+                float cmin[kBVHWidth][3], cmax[kBVHWidth][3];
+                for (int c = 0; c < nk; c++) {
+                    for (int a = 0; a < 3; a++) {
+                        cmin[c][a] = kids[c] >= 0 ? bn[kids[c]].box[a] : leafBox(~kids[c], a);
+                        cmax[c][a] = kids[c] >= 0 ? bn[kids[c]].box[3 + a] : leafBox(~kids[c], 3 + a);
+                    }
+                }
+                QBVHNode node;
+                quantizeNode(node, nk, cmin, cmax);
+                for (int c = 0; c < nk; c++) {
+                    node.triSize[c] = 0;
+                    if (kids[c] < 0) {
+                        node.childrenIdx[c] = 0x80000000u | (u32)keys[~kids[c]];
+                    } else {
+                        const int id = atomicAdd(&s_count, 1);
+                        bn[id].wideBin = kids[c];
+                        bn[id].wideDepth = level + 1;
+                        atomicMax(&s_depth, level + 1);
+                        node.childrenIdx[c] = (u32)id;
+                    }
+                }
+                out[k] = node;
+            }
+            __syncthreads();
+            done = count_now;
+        }
+        if (threadIdx.x == 0) {
+            R.tlasNodeCounts[w] = s_count;
+            recordTLASDepth(S, R, w, n, s_depth);
+        }
+        __syncthreads();
+    }
 }
 
 // ---- ray casting ------------------------------------------------------------------------------
@@ -524,9 +947,6 @@ struct RayHit {
     int instance;           // gather index inside the world, -1: miss
     int triangle;           // triangle index inside the instance's mesh
 };
-
-constexpr int kTraceStack = 48;     // TLAS + BLAS entries of one ray
-constexpr int kFlatInstances = 64;
 
 __device__ __forceinline__ float safeRcp(float x)
 {
@@ -899,9 +1319,10 @@ renderRaycastKernel(EngineState *Sp)
     for (i32 v = blockIdx.y; v < num_views; v += gridDim.y) {
         const RenderView view = R.views[v];
         const i32 w = view.worldIDX;
-        const QBVHNode *tlas = R.tlasNodes + (size_t)w * R.maxInstancesPerWorld;
+        const i32 instance_offset = R.instanceOffsets[w];
+        const QBVHNode *tlas = R.tlasNodes + instance_offset;
         const i32 tlas_nodes = R.tlasNodeCounts[w];
-        const RenderInstance *instances = R.instances + (size_t)w * R.maxInstancesPerWorld;
+        const RenderInstance *instances = R.instances + instance_offset;
         const i32 num_instances = R.instanceCounts[w];
         const RenderLight *lights = R.lights + (size_t)w * kMaxLightsPerWorld;
         const i32 num_lights = R.lightCounts[w];
@@ -1238,15 +1659,10 @@ bool renderHostAfterRegistry(Executor *ex, std::string *err)
     R.rgbCol = col(R.outputArchetype, R.cidRGB);
     R.depthCol = col(R.outputArchetype, R.cidDepth);
     R.lightCol = col(R.lightArchetype, R.cidLightDesc);
-    {
-        const char *v = getenv("MADRONA_B200_MAX_INSTANCES_PER_WORLD");
-        int cap = (v && *v) ? atoi(v) : 128;
-        R.maxInstancesPerWorld = std::min(std::max(cap, 8), 512);
-    }
     // the output table may grow (during world construction or between steps): the view
     // list covers every row it can ever have, so no view is left unrendered
     R.maxViews = (i32)ex->maxRows[R.outputArchetype];
-    rh->tlasSmem = tlasScratchBytes(R.maxInstancesPerWorld);
+    rh->tlasSmem = tlasScratchBytes(kWarpTLASInstances);
     cudaFuncSetAttribute(renderBuildTLASKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rh->tlasSmem);
 
     // light carriers: archetypes with LightCarrier + Position + every LightDesc* component
@@ -1282,10 +1698,11 @@ bool renderHostAfterRegistry(Executor *ex, std::string *err)
         return true;
     };
     const size_t W = S.numWorlds;
-    if (!alloc((void **)&R.instances, sizeof(RenderInstance) * W * R.maxInstancesPerWorld) ||
-        !alloc((void **)&R.instanceCounts, sizeof(i32) * W) ||
-        !alloc((void **)&R.tlasNodes, sizeof(QBVHNode) * W * R.maxInstancesPerWorld) ||
+    if (!alloc((void **)&R.instanceCounts, sizeof(i32) * W) ||
+        !alloc((void **)&R.instanceOffsets, sizeof(i32) * W) ||
         !alloc((void **)&R.tlasNodeCounts, sizeof(i32) * W) ||
+        !alloc((void **)&R.tlasDepths, sizeof(i32) * W) ||
+        !alloc((void **)&R.largeWorlds, sizeof(i32) * W) ||
         !alloc((void **)&R.lights, sizeof(RenderLight) * W * kMaxLightsPerWorld) ||
         !alloc((void **)&R.lightCounts, sizeof(i32) * W) ||
         (R.debugHits && !alloc((void **)&R.hitIDs, sizeof(i32) * 2 * (size_t)R.maxViews * R.resolution *
@@ -1294,19 +1711,59 @@ bool renderHostAfterRegistry(Executor *ex, std::string *err)
         *err = "render buffers allocation failed";
         return false;
     }
+    // instance list, TLAS nodes and large-world scratch: address ranges for every row the
+    // renderable tables can grow to, memory for the rows they have (renderEnsureCapacity)
+    uint64_t max_rows = 0;
+    for (u32 i = 0; i < R.numRenderArchetypes; i++) max_rows += (uint64_t)ex->maxRows[R.renderables[i].archetype];
+    max_rows = std::max<uint64_t>(std::min<uint64_t>(max_rows, 0x7fffff00ull), 1);
+    if (!vmReserve(ex->gpu, &rh->instanceRange, sizeof(RenderInstance) * max_rows, 0, err) ||
+        !vmReserve(ex->gpu, &rh->nodeRange, sizeof(QBVHNode) * max_rows, 0, err) ||
+        !vmReserve(ex->gpu, &rh->keyRange, sizeof(unsigned long long) * max_rows, 0, err) ||
+        !vmReserve(ex->gpu, &rh->buildRange, sizeof(TLASBuildNode) * max_rows, 0, err)) {
+        return false;
+    }
+    R.instances = (RenderInstance *)rh->instanceRange.base;
+    R.tlasNodes = (QBVHNode *)rh->nodeRange.base;
+    R.tlasKeys = (unsigned long long *)rh->keyRange.base;
+    R.tlasBuild = (TLASBuildNode *)rh->buildRange.base;
+    R.instanceCapacity = 0;
     cudaMemcpy(rh->dRender, &R, sizeof(RenderState), cudaMemcpyHostToDevice);
+    return renderEnsureCapacity(ex, err);
+}
+
+bool renderEnsureCapacity(Executor *ex, std::string *err)
+{
+    RenderHost *rh = ex->render;
+    if (!rh || !rh->active) return true;
+    RenderState &R = rh->hRender;
+    int64_t rows = 0;
+    for (u32 i = 0; i < R.numRenderArchetypes; i++) rows += ex->hState->tables[R.renderables[i].archetype].capacity;
+    rows = std::max<int64_t>(std::min<int64_t>(rows, 0x7fffff00ll), 1);
+    if (rows <= R.instanceCapacity) return true;
+    const size_t r = (size_t)rows;
+    if (!vmGrow(ex->gpu, &rh->instanceRange, sizeof(RenderInstance) * r, err) ||
+        !vmGrow(ex->gpu, &rh->nodeRange, sizeof(QBVHNode) * r, err) ||
+        !vmGrow(ex->gpu, &rh->keyRange, sizeof(unsigned long long) * r, err) ||
+        !vmGrow(ex->gpu, &rh->buildRange, sizeof(TLASBuildNode) * r, err)) {
+        *err = "render instance list: " + *err;
+        return false;
+    }
+    R.instanceCapacity = (i32)rows;
+    cudaMemcpy(&rh->dRender->instanceCapacity, &R.instanceCapacity, sizeof(i32), cudaMemcpyHostToDevice);
     return true;
 }
 
 void renderHostDestroy(Executor *ex)
 {
-    delete ex->render;
+    RenderHost *rh = ex->render;
+    if (rh) {
+        vmRelease(&rh->instanceRange);
+        vmRelease(&rh->nodeRange);
+        vmRelease(&rh->keyRange);
+        vmRelease(&rh->buildRange);
+    }
+    delete rh;
     ex->render = nullptr;
-}
-
-__global__ void renderResetCountsKernel(EngineState *Sp)
-{
-    Sp->render->totalNumInstances = 0;
 }
 
 bool renderEnqueuePrepare(Executor *ex, cudaStream_t s, std::string *err)
@@ -1316,7 +1773,8 @@ bool renderEnqueuePrepare(Executor *ex, cudaStream_t s, std::string *err)
     (void)err;
     const RenderState &R = rh->hRender;
     const unsigned W = ex->hState->numWorlds;
-    renderResetCountsKernel<<<1, 1, 0, s>>>(ex->dState);
+    renderCountInstancesKernel<<<(W * 32 + 127) / 128, 128, 0, s>>>(ex->dState);
+    renderScanInstancesKernel<<<1, 1024, 0, s>>>(ex->dState);
     renderGatherInstancesKernel<<<(W * 32 + 127) / 128, 128, 0, s>>>(ex->dState);
     // lights: carriers refresh their light entities, the light table is brought into
     // world order (no-op when clean), then listed per world
@@ -1335,6 +1793,11 @@ bool renderEnqueuePrepare(Executor *ex, cudaStream_t s, std::string *err)
     dim3 grid((unsigned)std::min((max_cap + 255) / 256, ex->numSMs * 4), std::max(R.numViewArchetypes, 1u));
     renderGatherViewsKernel<<<grid, 256, 0, s>>>(ex->dState);
     renderBuildTLASKernel<<<W, 32, rh->tlasSmem, s>>>(ex->dState);
+    // the step graph is captured once: the large-world builder's grid cannot follow the
+    // per-step count, so its blocks take worlds by ticket and leave when the list is empty
+    // (one block per SM: at 84 registers a second 512-thread block is not resident)
+    renderBuildLargeTLASKernel<<<std::max(1u, std::min(W, (unsigned)ex->numSMs)), kLargeTLASThreads, 0, s>>>(
+        ex->dState);
     return true;
 }
 
@@ -1344,17 +1807,17 @@ void *renderDebugHitBuffer(Executor *ex)
     return (rh && rh->active) ? (void *)rh->hRender.hitIDs : nullptr;
 }
 
-void *renderDebugBuffer(Executor *ex, int which, int64_t *stride_out)
+void *renderDebugBuffer(Executor *ex, int which)
 {
     RenderHost *rh = ex->render;
     if (!rh || !rh->active) return nullptr;
     const RenderState &R = rh->hRender;
-    *stride_out = R.maxInstancesPerWorld;
     switch (which) {
     case 1: return R.tlasNodes;
     case 2: return R.tlasNodeCounts;
     case 3: return R.instances;
     case 4: return R.instanceCounts;
+    case 5: return R.instanceOffsets;
     default: return nullptr;
     }
 }

@@ -216,6 +216,8 @@ enum ErrorFlags : u32 {
     ErrRegistry = 1u << 5,
     ErrPhysicsOverflow = 1u << 6,
     ErrRenderAsset = 1u << 7,          // a material names a texture the render config does not have
+    ErrRenderCapacity = 1u << 8,       // more visible instances than the instance list holds
+    ErrRenderTLASDepth = 1u << 9,      // a world's TLAS is too deep for the ray caster's stack
 };
 
 }

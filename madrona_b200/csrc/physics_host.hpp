@@ -19,8 +19,10 @@ bool renderHostCreate(Executor *ex, const mb2_render_config *rc, std::string *er
 bool renderHostAfterRegistry(Executor *ex, std::string *err);
 void renderHostDestroy(Executor *ex);
 bool renderEnqueuePrepare(Executor *ex, cudaStream_t s, std::string *err);
+// after a renderable table grew: map instance-list rows for its new capacity
+bool renderEnsureCapacity(Executor *ex, std::string *err);
 void *renderDebugHitBuffer(Executor *ex);
-void *renderDebugBuffer(Executor *ex, int which, int64_t *stride_out);
+void *renderDebugBuffer(Executor *ex, int which);
 uint64_t renderBytesPerFrame(Executor *ex, int64_t num_views);
 // algorithmic bytes of one launch of a physics node + a short name (profiling)
 uint64_t physicsNodeBytes(Executor *ex, const NodeRecord &rec, const char **name, int64_t *rows);

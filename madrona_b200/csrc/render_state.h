@@ -100,11 +100,22 @@ struct RenderState {
     ViewArchetype viewers[kMaxRenderArchetypes];
     i32 rgbCol, depthCol;
 
-    RenderInstance *instances;      // [numWorlds][maxInstancesPerWorld], gather order
-    i32 *instanceCounts;            // [numWorlds]
-    i32 maxInstancesPerWorld;
-    QBVHNode *tlasNodes;            // [numWorlds][maxInstancesPerWorld], node 0 = root
-    i32 *tlasNodeCounts;            // [numWorlds]
+    // Instances are one world-major list: world w's, in gather order, start at
+    // instanceOffsets[w] (exclusive scan of instanceCounts).  The list, the TLAS nodes and
+    // the large-world builder's scratch have one entry per row of the renderable tables
+    // (instanceCapacity), mapped behind address ranges that grow with those tables.
+    RenderInstance *instances;      // [instanceCapacity]
+    i32 *instanceCounts;            // [numWorlds] visible renderables
+    i32 *instanceOffsets;           // [numWorlds]
+    i32 instanceCapacity;
+    QBVHNode *tlasNodes;            // [instanceCapacity]; world w's tree at instanceOffsets[w], node 0 = root
+    i32 *tlasNodeCounts;            // [numWorlds] (<= max(1, n - 1))
+    i32 *tlasDepths;                // [numWorlds] levels of 4-wide nodes (0: no tree)
+    unsigned long long *tlasKeys;   // [instanceCapacity] large-world builder: sorted Morton keys
+    struct TLASBuildNode *tlasBuild;   // [instanceCapacity] large-world builder: binary / wide nodes
+    i32 *largeWorlds;               // [numWorlds] worlds above the warp builder's size, world order
+    u32 numLargeWorlds;
+    u32 largeTicket;                // next entry of largeWorlds a builder block takes
     RenderLight *lights;            // [numWorlds][kMaxLightsPerWorld]
     i32 *lightCounts;               // [numWorlds]
     i32 lightCol;

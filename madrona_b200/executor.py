@@ -473,21 +473,25 @@ class MWCudaExecutor:
         return torch.as_tensor(view, device=f"cuda:{self.gpu_id}")
 
     def renderDebugStructures(self):
-        """(tlas_nodes u8 [W, cap, 60], tlas_counts [W], instances u8 [W, cap, 76], instance_counts [W])
-        of the last render-prepare (test hook)."""
+        """(tlas_nodes u8 [N, 60], tlas_counts [W], instances u8 [N, 76], instance_counts [W],
+        instance_offsets [W]) of the last render-prepare (test hook).  Compact layouts: world w's
+        instances and TLAS nodes (node 0 = root) start at instance_offsets[w]; N = visible
+        instances of all worlds."""
         import torch
-        cap = ctypes.c_int64(0)
-        out = []
-        for which, (bytes_per, counts) in ((1, (60, False)), (2, (4, True)), (3, (76, False)), (4, (4, True))):
-            p = self._lib.mb2_render_debug_buffer(self._h, which, ctypes.byref(cap))
+        stride = ctypes.c_int64(0)
+
+        def fetch(which, shape, typestr):
+            p = self._lib.mb2_render_debug_buffer(self._h, which, ctypes.byref(stride))
             if not p:
                 raise MadronaB200Error("no renderer")
-            if counts:
-                view = _CudaView(p, (self.num_worlds,), "<i4")
-            else:
-                view = _CudaView(p, (self.num_worlds, cap.value, bytes_per), "|u1")
-            out.append(torch.as_tensor(view, device=f"cuda:{self.gpu_id}").cpu().numpy())
-        return out
+            return torch.as_tensor(_CudaView(p, shape, typestr), device=f"cuda:{self.gpu_id}").cpu().numpy()
+
+        W = self.num_worlds
+        ncount, icount, offsets = fetch(2, (W,), "<i4"), fetch(4, (W,), "<i4"), fetch(5, (W,), "<i4")
+        total = int(offsets[-1] + icount[-1])
+        nodes = fetch(1, (max(total, 1), 60), "|u1")[:total]
+        inst = fetch(3, (max(total, 1), 76), "|u1")[:total]
+        return nodes, ncount, inst, icount, offsets
 
     def peerGather(self, slots, shapes, dtypes, world_size: int, rank: int):
         """NVLink peer-store gather of fixed-size exported columns across the ranks of a

@@ -10,13 +10,13 @@ W, P = 2, 100
 ex = make_executor("gallery", W, num_props=P, seed=5, resolution=16, rgbd=True)
 step = ex.buildLaunchGraphAllTaskGraphs()
 ex.run(step)
-nodes_raw, ncount, inst_raw, icount = ex.renderDebugStructures()
-print("instance counts", icount, "tlas node counts", ncount)
+nodes_raw, ncount, inst_raw, icount, offsets = ex.renderDebugStructures()
+print("instance counts", icount, "offsets", offsets, "tlas node counts", ncount)
 for w in range(W):
-    n = int(icount[w]); k = int(ncount[w])
-    inst = inst_raw[w, :n].copy().view(np.float32).reshape(n, 19)
+    n = int(icount[w]); k = int(ncount[w]); o = int(offsets[w])
+    inst = inst_raw[o:o + n].copy().view(np.float32).reshape(n, 19)
     lo_i, hi_i = inst[:, 13:16], inst[:, 16:19]
-    nodes = _decode_nodes(nodes_raw[w, :k])
+    nodes = _decode_nodes(nodes_raw[o:o + k])
     seen = np.zeros(n, dtype=int)
     stack = [0]; visited = 0; bad = 0
     while stack and visited < 4 * max(k, 1):

@@ -270,6 +270,24 @@ SIMS: Dict[str, SimDesc] = {
         render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_render_config(
             int(cfg.get("resolution", 40)), bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0))),
     ),
+    # GPU only: the gallery built with -DGALLERY_PER_WORLD=1: props[w] props in world w (every
+    # 17th hidden, as in the gallery), layouts[w] 0 scattered / 1 clustered (deep Morton tree)
+    "gallery_sized": SimDesc(
+        name="gallery_sized",
+        sources=[os.path.join(_ROOT, "gallery", "sim.cpp")],
+        num_exports=10,
+        num_taskgraphs=1,
+        inputs=[],
+        outputs=[],
+        pack_config=lambda cfg: struct.pack("<II", 0, 5),
+        pack_init=lambda w, cfg: struct.pack("<III", int(cfg.get("seed", 0)) + w, int(cfg["props"][w]),
+                                             int(cfg["layouts"][w]) if cfg.get("layouts") else 0),
+        oracle_extra=lambda cfg: [],
+        defaults={"props": [100], "layouts": None, "seed": 0, "resolution": 40, "rgbd": True},
+        compile_flags=["-DGALLERY_PER_WORLD=1"],
+        render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_render_config(
+            int(cfg.get("resolution", 40)), bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0))),
+    ),
     # GPU only: the gallery sim with uvs and textured materials (tests/test_render_textures.py);
     # same sources and flags, so it shares the gallery's simulator module
     "gallery_textured": SimDesc(

@@ -51,9 +51,16 @@ Sim::Sim(Engine &ctx, const Config &cfg, const WorldInit &init)
 {
     RenderingSystem::init(ctx, nullptr);
     const uint32_t ground_obj = cfg.numMeshes - 1;
+#if defined(GALLERY_PER_WORLD)
+    const uint32_t num_props = init.numProps;
+    const bool clustered = init.layout == Layout::Clustered;
+#else
+    const uint32_t num_props = cfg.numProps;
+    const bool clustered = false;
+#endif
 
     // the ground: one big quad
-    {
+    if (num_props > 0) {
         Entity e = ctx.makeEntity<Prop>();
         ctx.get<Position>(e) = Vector3 { 0, 0, 0 };
         ctx.get<Rotation>(e) = Quat { 1, 0, 0, 0 };
@@ -64,12 +71,21 @@ Sim::Sim(Engine &ctx, const Config &cfg, const WorldInit &init)
         ctx.get<Spin>(e).phase = 0.f;
         RenderingSystem::makeEntityRenderable(ctx, e);
     }
-    for (uint32_t i = 1; i < cfg.numProps; i++) {
+    for (uint32_t i = 1; i < num_props; i++) {
         Entity e = ctx.makeEntity<Prop>();
         float x = (rng.sampleUniform() - 0.5f) * 24.f;
         float y = (rng.sampleUniform() - 0.5f) * 24.f;
         float z = 0.6f + rng.sampleUniform() * 2.5f;
         float s = 0.5f + rng.sampleUniform();
+        if (clustered) {
+            // prop i sits at radius 6 * 0.93^i around (0, 0, 2), at 1/8 of that size
+            const float r = 6.f * powf(0.93f, (float)i);
+            const float a = 2.39996f * (float)i;
+            x = r * cosf(a);
+            y = r * sinf(a);
+            z = 2.f + 0.3f * r;
+            s = 0.125f * r;
+        }
         ctx.get<Position>(e) = Vector3 { x, y, z };
         Quat q { rng.sampleUniform() - 0.5f, rng.sampleUniform() - 0.5f, rng.sampleUniform() - 0.5f,
                  rng.sampleUniform() + 0.1f };

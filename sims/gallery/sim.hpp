@@ -58,7 +58,17 @@ struct Config {
     uint32_t numMeshes;     // object IDs 0 .. numMeshes - 2 are props, numMeshes - 1 is the ground
 };
 
+#if defined(GALLERY_PER_WORLD)
+// build variant "gallery_sized": every world says how many props it has (0: not even the
+// ground) and how they are laid out
+enum class Layout : uint32_t {
+    Scattered,      // as the gallery: uniform over the floor
+    Clustered,      // a spiral at geometrically shrinking radii and sizes (deep Morton trees)
+};
+struct WorldInit { uint32_t seed; uint32_t numProps; Layout layout; };
+#else
 struct WorldInit { uint32_t seed; };
+#endif
 
 class Engine;
 
