@@ -15,6 +15,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <algorithm>
+#include <cxxabi.h>
 
 namespace mb2 {
 
@@ -67,6 +68,8 @@ static std::string describeErrors(uint32_t flags, uint32_t archetype)
     if (flags & ErrTmpOverflow) s += "tmp allocator overflow (raise MADRONA_B200_TMP_BYTES) ";
     if (flags & ErrPersistOverflow) s += "persistent arena overflow (raise MADRONA_B200_PERSIST_BYTES) ";
     if (flags & ErrTooManyNodes) s += "too many taskgraph nodes ";
+    if (flags & ErrTooManyNodeDatas) s += "too many custom node datas (constructNodeData; at most " +
+        std::to_string(kMaxNodeDatas) + ") ";
     if (flags & ErrRegistry) s += "ECS registration error (unregistered component, too many types, bad export slot) ";
     if (flags & ErrPhysicsOverflow) s += "physics buffer overflow ";
     if (flags & ErrRenderAsset) s += "render asset error (a material's textureIdx is not below "
@@ -510,6 +513,9 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
     if (!pullState(ex)) return false;
     S.numEntitySlots = (int32_t)(next_block * kIDsPerCache);
     S.initPass = 2;
+    // custom node data (after every other allocation of the executor, which therefore keeps
+    // its placement); one spare slot past the limit absorbs overflowing constructs
+    if (!devAlloc(ex, (void **)&S.nodeData, (size_t)(kMaxNodeDatas + 1) * kNodeDataBytes)) return false;
     if (!pushState(ex)) return false;
 
     // ---- phase 4: setupTasks on the device (1 thread)
@@ -517,10 +523,15 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
     if (!pullState(ex)) return false;
     if (!checkDeviceErrors(ex, "setupTasks")) return false;
 
-    // resolve ParallelFor records to kernels
+    // resolve ParallelFor and custom-node records to kernels
     for (uint32_t n = 0; n < S.numNodes; n++) {
         NodeRecord &r = S.nodes[n];
-        if (r.kind != NodeUserParallelFor) continue;
+        if (r.kind != NodeUserParallelFor && r.kind != NodeUserFn) continue;
+        if (r.kind == NodeUserFn && (r.userFn.threadsPerInvocation == 0 || 256 % r.userFn.threadsPerInvocation != 0)) {
+            setError("taskgraph node " + std::to_string(n) + ": addNodeFn num_threads_per_invocation = " +
+                     std::to_string(r.userFn.threadsPerInvocation) + "; it must be at least 1 and divide 256");
+            return false;
+        }
         uint64_t addr = ((uint64_t)r.component << 32) | r.kernelID;
         size_t k = 0;
         for (; k < ex->nodeMetaAddrs.size(); k++) {
@@ -534,6 +545,7 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
     }
     MB2_CUDA(cudaMemcpy(ex->dState->nodes, S.nodes, sizeof(NodeRecord) * S.numNodes,
                         cudaMemcpyHostToDevice));
+    ex->nodeKernelGrid.assign(ex->nodeKernels.size(), 0);
 
     // ---- phase 5: bring every table into world order so exported columns are
     // world-major from step 0 (the CPU backend's layout, src/core/state.cpp:576-619)
@@ -570,6 +582,18 @@ static void destroyExecutor(Executor *ex)
 
 // ---- launch graphs -----------------------------------------------------------
 
+// Blocks of 256 threads that node kernel k keeps resident on the whole device, queried once
+static bool persistentGrid(Executor *ex, uint32_t k, unsigned *grid)
+{
+    if (ex->nodeKernelGrid[k] == 0) {
+        int per_sm = 0;
+        MB2_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void *)ex->nodeKernels[k], 256, 0));
+        ex->nodeKernelGrid[k] = (uint32_t)ex->numSMs * (uint32_t)std::max(per_sm, 1);
+    }
+    *grid = ex->nodeKernelGrid[k];
+    return true;
+}
+
 static bool enqueueNode(Executor *ex, uint32_t node_idx, cudaStream_t s)
 {
     EngineState &S = *ex->hState;
@@ -581,6 +605,22 @@ static bool enqueueNode(Executor *ex, uint32_t node_idx, cudaStream_t s)
         uint64_t blocks = (threads + 255) / 256;
         uint64_t max_blocks = (uint64_t)ex->numSMs * 8;
         unsigned grid = (unsigned)std::max<uint64_t>(1, std::min(blocks, max_blocks));
+        const NodeRecord *drec = &ex->dState->nodes[node_idx];
+        void *args[1] = { (void *)&drec };
+        MB2_CUDA(cudaLaunchKernel((const void *)ex->nodeKernels[r.kernelID], dim3(grid), dim3(256), args, 0, s));
+        return true;
+    }
+    case NodeUserFn: {
+        // fixed counts: just enough blocks, at most the persistent grid; dynamic counts: the
+        // persistent grid, after the count is latched (a count of 0 launches blocks that exit)
+        unsigned grid = 0;
+        if (!persistentGrid(ex, r.kernelID, &grid)) return false;
+        if (r.userFn.fixedCount > 0) {
+            const uint64_t blocks = ((uint64_t)r.userFn.fixedCount * r.userFn.threadsPerInvocation + 255) / 256;
+            grid = (unsigned)std::min<uint64_t>(blocks, grid);
+        } else {
+            launchLatchNodeCount(ex, node_idx, s);
+        }
         const NodeRecord *drec = &ex->dState->nodes[node_idx];
         void *args[1] = { (void *)&drec };
         MB2_CUDA(cudaLaunchKernel((const void *)ex->nodeKernels[r.kernelID], dim3(grid), dim3(256), args, 0, s));
@@ -827,6 +867,47 @@ static LaunchGraph *buildGraph(Executor *ex, const uint32_t *ids, uint32_t n, co
 
 // ---- per-node profiling ------------------------------------------------------
 
+// "ns::Node::run" from nodeKern<FnNode<ns::Node, &ns::Node::run>>'s mangled name
+static std::string customNodeName(const std::string &mangled)
+{
+    int status = 0;
+    char *d = abi::__cxa_demangle(mangled.c_str(), nullptr, nullptr, &status);
+    if (!d) return mangled;
+    std::string full(d);
+    free(d);
+    size_t p = full.find("FnNode<");
+    if (p == std::string::npos) return full;
+    p += 7;
+    size_t comma = std::string::npos, end = full.size();
+    int depth = 0;
+    for (size_t i = p; i < full.size(); i++) {
+        const char c = full[i];
+        if (c == '<' || c == '(') depth++;
+        else if (c == ')') depth--;
+        else if (c == '>') {
+            if (depth == 0) { end = i; break; }
+            depth--;
+        } else if (c == ',' && depth == 0) {
+            comma = i;
+        }
+    }
+    std::string fn = full.substr(comma == std::string::npos ? p : comma + 1,
+                                 end - (comma == std::string::npos ? p : comma + 1));
+    while (!fn.empty() && (fn[0] == ' ' || fn[0] == '&')) fn.erase(0, 1);
+    while (!fn.empty() && fn.back() == ' ') fn.pop_back();
+    // a free or static function: "(void ns::f<T>(T*, int))" -> "ns::f<T>"
+    if (fn.size() > 2 && fn.front() == '(' && fn.back() == ')') {
+        fn = fn.substr(1, fn.size() - 2);
+        if (fn.rfind("void ", 0) == 0) fn.erase(0, 5);
+        int d = 0;
+        for (size_t i = fn.size(); i-- > 0;) {
+            if (fn[i] == ')') d++;
+            else if (fn[i] == '(' && --d == 0) { fn.erase(i); break; }
+        }
+    }
+    return fn;
+}
+
 struct NodeProfile {
     double ms = 0;
     double bytes = 0;
@@ -900,7 +981,9 @@ static int64_t profileNodes(Executor *ex, const uint32_t *ids, uint32_t n, uint3
             p.samples++;
             const TableDesc &t = tables[r.archetype < S.numArchetypes ? r.archetype : 0];
             double rows = t.numRows, bytes = 0;
-            if (r.kind == NodeUserParallelFor) {
+            if (r.kind == NodeUserFn) {
+                rows = r.userFn.fixedCount;   // invocations; 0 for a dynamic count
+            } else if (r.kind == NodeUserParallelFor) {
                 double per_row = 4;   // WorldID
                 for (int c = 0; c < r.numCols; c++) per_row += t.columnBytes[r.cols[c]];
                 bytes = rows * per_row;
@@ -930,12 +1013,12 @@ static int64_t profileNodes(Executor *ex, const uint32_t *ids, uint32_t n, uint3
     }
 
     static const char *kind_names[] = { "parallel_for", "sort_archetype", "compact_archetype",
-                                        "clear_tmp", "reset_tmp_alloc", "recycle_entities" };
+                                        "clear_tmp", "reset_tmp_alloc", "recycle_entities", "custom" };
     std::string js = "[";
     for (size_t k = 0; k < order.size(); k++) {
         const NodeRecord &r = S.nodes[order[k]];
         const NodeProfile &p = prof[k];
-        const char *kn = r.kind < 6 ? kind_names[r.kind] : "physics";
+        const char *kn = r.kind <= NodeUserFn ? kind_names[r.kind] : "physics";
         if (r.kind >= NodePhysBroadphaseUpdate) {
             int64_t rows;
             physicsNodeBytes(ex, r, &kn, &rows);
@@ -950,6 +1033,9 @@ static int64_t profileNodes(Executor *ex, const uint32_t *ids, uint32_t n, uint3
                 size_t b = m.find("ERS", a);
                 name += ":" + m.substr(a + 6, b == std::string::npos ? 32 : b - a - 6);
             }
+        }
+        if (r.kind == NodeUserFn && r.kernelID < ex->jit.nodeKernels.size()) {
+            name += ":" + customNodeName(ex->jit.nodeKernels[r.kernelID]);
         }
         double s = p.samples ? 1.0 / (double)p.samples : 0.0;
         char buf[512];

@@ -26,6 +26,7 @@ struct Executor {
     cudaKernel_t initECS = nullptr, initWorlds = nullptr, initTasks = nullptr;
     std::vector<cudaKernel_t> nodeKernels;
     std::vector<uint64_t> nodeMetaAddrs;
+    std::vector<uint32_t> nodeKernelGrid;   // resident blocks of each node kernel (0: not queried yet)
 
     EngineState *dState = nullptr;     // device
     EngineState *hState = nullptr;     // host mirror (registry, nodes, table descs)
@@ -70,6 +71,7 @@ void setError(const std::string &msg);
 // ---- ahead-of-time engine kernels (kernels_core.cu / kernels_sort.cu) -----
 void launchClearTmp(Executor *ex, uint32_t archetype, cudaStream_t s);
 void launchResetTmpAlloc(Executor *ex, cudaStream_t s);
+void launchLatchNodeCount(Executor *ex, uint32_t node, cudaStream_t s);
 void launchStatusCopy(Executor *ex, cudaStream_t s);
 void launchFillSingletons(Executor *ex, cudaStream_t s);
 

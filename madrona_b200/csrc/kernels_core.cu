@@ -65,6 +65,21 @@ __global__ void fillSingletonsKernel(EngineState *S)
     }
 }
 
+// A dynamic-count custom node reads its count once, after its dependencies finished and
+// before any invocation runs (reference: src/mw/device/taskgraph.cpp:132-140), so a node
+// may change its own numDynamicInvocations while it runs.  NodeBase sits at the start of
+// the node data.
+__global__ void latchNodeCountKernel(EngineState *S, uint32_t node)
+{
+    NodeRecord &r = S->nodes[node];
+    r.userFn.latchedCount = *(const uint32_t *)(S->nodeData + (size_t)r.userFn.dataIdx * kNodeDataBytes);
+}
+
+void launchLatchNodeCount(Executor *ex, uint32_t node, cudaStream_t s)
+{
+    latchNodeCountKernel<<<1, 1, 0, s>>>(ex->dState, node);
+}
+
 void launchClearTmp(Executor *ex, uint32_t archetype, cudaStream_t s)
 {
     int grid = (int)std::min<uint32_t>((ex->hState->numWorlds + 255) / 256, (uint32_t)ex->numSMs * 2);

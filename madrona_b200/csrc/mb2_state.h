@@ -34,6 +34,8 @@ constexpr int kMaxNodes = 1024;
 constexpr int kMaxNodeCols = 16;
 constexpr int kMaxNodeDeps = 8;
 constexpr int kMaxTaskGraphs = 8;
+constexpr int kMaxNodeDatas = 1024;    // custom node data slots (TaskGraphBuilder::constructNodeData)
+constexpr int kNodeDataBytes = 256;    // bytes and alignment of one slot (reference: taskgraph.hpp:36-40)
 constexpr int kIDsPerCache = 64;       // reference: include/madrona/impl/id_map.hpp:132
 constexpr i32 kIDSentinel = (i32)0xFFFFFFFF;
 constexpr u32 kBundleMask = 0x80000000u;  // reference: include/madrona/state.hpp:401
@@ -114,6 +116,7 @@ enum NodeKind : u32 {
     NodeClearTmp = 3,
     NodeResetTmpAlloc = 4,
     NodeRecycleEntities = 5,
+    NodeUserFn = 6,                  // TaskGraphBuilder::addNodeFn (custom node types)
     // engine-owned systems (ahead-of-time kernels)
     NodePhysBroadphaseUpdate = 16,   // leaf AABB update + refit
     NodePhysBVHRebuild = 17,
@@ -133,6 +136,16 @@ enum NodeKind : u32 {
     NodeRenderPrepare = 32,
 };
 
+// NodeUserFn: the node's data slot, its fixed invocation count (0: dynamic, the count is
+// latched into latchedCount from the data's NodeBase::numDynamicInvocations right before
+// the launch) and its threads per invocation
+struct UserFnParams {
+    u32 dataIdx;
+    u32 fixedCount;
+    u32 threadsPerInvocation;
+    u32 latchedCount;
+};
+
 struct NodeRecord {
     u32 kind;
     u32 taskgraph;
@@ -140,7 +153,10 @@ struct NodeRecord {
     u32 archetype;
     u32 component;         // sort key component
     i32 numCols;
-    i32 cols[kMaxNodeCols];
+    union {
+        i32 cols[kMaxNodeCols];
+        UserFnParams userFn;   // NodeUserFn
+    };
     u32 numDeps;
     u32 deps[kMaxNodeDeps];
     u32 userTag;
@@ -205,6 +221,10 @@ struct EngineState {
     // ---- engine-owned systems
     PhysicsState *physics;
     RenderState *render;
+
+    // ---- custom node data (TaskGraphBuilder::constructNodeData)
+    char *nodeData;                  // [kMaxNodeDatas + 1] slots of kNodeDataBytes; the last one
+    u32 numNodeDatas;                // absorbs constructs past the limit (ErrTooManyNodeDatas)
 };
 
 enum ErrorFlags : u32 {
@@ -218,6 +238,7 @@ enum ErrorFlags : u32 {
     ErrRenderAsset = 1u << 7,          // a material names a texture the render config does not have
     ErrRenderCapacity = 1u << 8,       // more visible instances than the instance list holds
     ErrRenderTLASDepth = 1u << 9,      // a world's TLAS is too deep for the ray caster's stack
+    ErrTooManyNodeDatas = 1u << 10,    // more custom node datas than kMaxNodeDatas
 };
 
 }

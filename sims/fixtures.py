@@ -58,6 +58,10 @@ def _grid_init(w, cfg):
     return struct.pack("<I", int(cfg.get("seed", 0)) + w)
 
 
+def _customnodes_init(w, cfg):
+    return struct.pack("<II", int(cfg.get("seed", 0)) + w, 1 if w % 7 == 3 else 0)
+
+
 def _room_cfg(cfg):
     return struct.pack("<QII", int(cfg.get("obj_mgr_ptr", 0)), int(cfg["episode_len"]),
                        int(cfg.get("grab_period", 0)))
@@ -392,6 +396,58 @@ SIMS: Dict[str, SimDesc] = {
         oracle_extra=lambda cfg: [int(cfg["grid_size"]), int(cfg["episode_len"]),
                                   int(cfg["init_items"]), int(cfg.get("seed", 0))],
         defaults={"grid_size": 8, "episode_len": 50, "init_items": 6, "seed": 0},
+    ),
+    # custom task-graph nodes: addNodeFn (fixed counts, 1 / 32 / 256 threads per invocation),
+    # addDynamicCountNode, addOneOffNode, node data, a second task graph (tests/test_custom_nodes.py);
+    # world w never has tokens when w % 7 == 3
+    "customnodes": SimDesc(
+        name="customnodes",
+        sources=[os.path.join(_ROOT, "customnodes", "sim.cpp")],
+        num_exports=8,
+        num_taskgraphs=2,
+        inputs=[],
+        outputs=[Slot(0, "world_sum", "uint32", (4,)), Slot(1, "coop", "uint32", (7,)),
+                 Slot(2, "census", "uint32", (4,)),
+                 Slot(3, "token_entity", "int32", (2,), dynamic=True),
+                 Slot(4, "token_val", "uint32", (1,), dynamic=True),
+                 Slot(5, "token_out", "uint32", (1,), dynamic=True)],
+        pack_config=lambda cfg: struct.pack("<IIII", 0, 0, 0, 0),
+        pack_init=_customnodes_init,
+        oracle_extra=lambda cfg: [int(cfg.get("seed", 0))],
+        defaults={"seed": 0},
+    ),
+    # GPU only: the same fixture with the ParallelForNode twin of its dynamic-count node
+    # (scripts/bench_custom_nodes.py); it computes the same columns
+    "customnodes_bench": SimDesc(
+        name="customnodes_bench",
+        sources=[os.path.join(_ROOT, "customnodes", "sim.cpp")],
+        num_exports=8,
+        num_taskgraphs=2,
+        inputs=[],
+        outputs=[Slot(0, "world_sum", "uint32", (4,)), Slot(1, "coop", "uint32", (7,)),
+                 Slot(5, "token_out", "uint32", (1,), dynamic=True)],
+        pack_config=lambda cfg: struct.pack("<IIII", 0, 0, 0, 0),
+        pack_init=_customnodes_init,
+        oracle_extra=lambda cfg: [],
+        defaults={"seed": 0},
+        compile_flags=["-DCUSTOMNODES_BENCH=1"],
+    ),
+    # GPU only: invocation probe -- a node with fixed count `count` (0: dynamic) and `threads`
+    # threads per invocation records its runs in 4096 rows (invocation i -> row i % 4096);
+    # dynamic=1 sets the count from a one-off node and has invocation 0 zero it while it runs
+    "customnodes_probe": SimDesc(
+        name="customnodes_probe",
+        sources=[os.path.join(_ROOT, "customnodes", "sim.cpp")],
+        num_exports=8,
+        num_taskgraphs=2,
+        inputs=[],
+        outputs=[Slot(6, "probe", "uint32", (14,), dynamic=True), Slot(7, "probe_info", "uint32", (2,))],
+        pack_config=lambda cfg: struct.pack("<IIII", int(cfg["count"]), int(cfg["threads"]),
+                                            int(cfg["dynamic"]), int(cfg["extra_node_datas"])),
+        pack_init=_customnodes_init,
+        oracle_extra=lambda cfg: [],
+        defaults={"count": 1, "threads": 1, "dynamic": 0, "extra_node_datas": 0, "seed": 0},
+        compile_flags=["-DCUSTOMNODES_PROBE=1"],
     ),
     "cartpole": SimDesc(
         name="cartpole",
