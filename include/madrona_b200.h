@@ -306,6 +306,35 @@ typedef struct mb2_rigid_body_assets {
 void mb2_object_manager_host_assets(const mb2_object_manager *mgr, mb2_rigid_body_assets *out);
 void mb2_object_manager_destroy(mb2_object_manager *mgr);
 
+/* ---- navigation meshes -----------------------------------------------------
+ * Role of the reference's host Navmesh::initFromPolygons (include/madrona/
+ * navmesh.hpp, src/common/navmesh.cpp) for a mesh that many worlds share:
+ * polygons (CCW vertex loops, fanned from their first index) in, the four
+ * arrays of a madrona::Navmesh out, bit-identical to the reference's, uploaded
+ * once to gpu_id (gpu_id < 0: host arrays only).  Bad input returns NULL and
+ * mb2_last_error() says why: a null array, no polygons, a polygon of fewer
+ * than 3 vertices, one running past num_idxs, or an index >= num_verts.
+ * mb2_navmesh_view returns a host copy of the 40-byte madrona::Navmesh that
+ * holds the device pointers, to copy into a simulator's Config (NULL without a
+ * GPU).  Executors adopt those pointers without owning them: destroy the
+ * navmesh after every executor that uses it. */
+typedef struct mb2_navmesh mb2_navmesh;
+typedef struct mb2_navmesh_arrays {
+    const float *vertices;              /* xyz per vertex */
+    const uint32_t *tri_indices;        /* 3 per triangle */
+    const uint32_t *tri_adjacency;      /* 3 per triangle, edge (a,b) (b,c) (c,a); 0xFFFFFFFF: none */
+    const void *alias_table;            /* Navmesh::AliasEntry {float tau; uint32_t alias} per triangle */
+    uint32_t num_verts;
+    uint32_t num_tris;
+} mb2_navmesh_arrays;
+mb2_navmesh *mb2_navmesh_create(const float *vertices_xyz, uint32_t num_verts,
+                                const uint32_t *poly_idxs, uint32_t num_idxs,
+                                const uint32_t *poly_offsets, const uint32_t *poly_sizes,
+                                uint32_t num_polys, int gpu_id);
+const void *mb2_navmesh_view(const mb2_navmesh *navmesh);
+void mb2_navmesh_host_arrays(const mb2_navmesh *navmesh, mb2_navmesh_arrays *out);
+void mb2_navmesh_destroy(mb2_navmesh *navmesh);
+
 /* ---- multi-GPU gather of exported columns (SURVEY.md 8e) ------------------
  * No reference counterpart (the reference is single-GPU, mw_gpu.hpp:122):
  * worlds shard across GPUs, one process per GPU, and the only exchange is the

@@ -19,6 +19,7 @@ from .executor import (  # noqa: F401
     MeshBVHData,
     MaterialData,
     RigidBodyAssets,
+    Navmesh,
     PeerGather,
 )
 from .tensor import (  # noqa: F401

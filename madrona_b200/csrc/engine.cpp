@@ -70,6 +70,8 @@ static std::string describeErrors(uint32_t flags, uint32_t archetype)
     if (flags & ErrTooManyNodes) s += "too many taskgraph nodes ";
     if (flags & ErrTooManyNodeDatas) s += "too many custom node datas (constructNodeData; at most " +
         std::to_string(kMaxNodeDatas) + ") ";
+    if (flags & ErrNavmeshPolygon) s += "navmesh polygon with fewer than 3 vertices "
+        "(Navmesh::initFromPolygons built nothing) ";
     if (flags & ErrRegistry) s += "ECS registration error (unregistered component, too many types, bad export slot) ";
     if (flags & ErrPhysicsOverflow) s += "physics buffer overflow ";
     if (flags & ErrRenderAsset) s += "render asset error (a material's textureIdx is not below "

@@ -239,6 +239,7 @@ enum ErrorFlags : u32 {
     ErrRenderCapacity = 1u << 8,       // more visible instances than the instance list holds
     ErrRenderTLASDepth = 1u << 9,      // a world's TLAS is too deep for the ray caster's stack
     ErrTooManyNodeDatas = 1u << 10,    // more custom node datas than kMaxNodeDatas
+    ErrNavmeshPolygon = 1u << 11,      // Navmesh::initFromPolygons got a polygon of fewer than 3 vertices
 };
 
 }

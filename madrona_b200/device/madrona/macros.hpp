@@ -21,8 +21,10 @@
 #define MADRONA_IMPORT
 #if defined(__CUDA_ARCH__) || defined(__CUDACC_RTC__)
 #define MB2_CLZ(v) __clz((int)(v))
+#define MB2_CLZLL(v) __clzll((long long)(v))
 #define MB2_POPC(v) __popc((unsigned)(v))
 #else
 #define MB2_CLZ(v) __builtin_clz(v)
+#define MB2_CLZLL(v) __builtin_clzll(v)
 #define MB2_POPC(v) __builtin_popcount(v)
 #endif

@@ -49,6 +49,10 @@ EXPORTED_SYMBOLS = [
     "mb2_object_manager_ptr",
     "mb2_object_manager_host_assets",
     "mb2_object_manager_destroy",
+    "mb2_navmesh_create",
+    "mb2_navmesh_view",
+    "mb2_navmesh_host_arrays",
+    "mb2_navmesh_destroy",
     "mb2_render_debug_hits",
     "mb2_render_debug_buffer",
     "mb2_peer_gather_create",
@@ -142,6 +146,12 @@ class _RigidBodyAssetsC(ctypes.Structure):
                 ("prim_offsets", ctypes.c_void_p), ("prim_counts", ctypes.c_void_p),
                 ("num_convex_hulls", ctypes.c_uint32), ("total_num_primitives", ctypes.c_uint32),
                 ("num_objs", ctypes.c_uint32)]
+
+
+class _NavmeshArraysC(ctypes.Structure):   # == mb2_navmesh_arrays
+    _fields_ = [("vertices", ctypes.c_void_p), ("tri_indices", ctypes.c_void_p),
+                ("tri_adjacency", ctypes.c_void_p), ("alias_table", ctypes.c_void_p),
+                ("num_verts", ctypes.c_uint32), ("num_tris", ctypes.c_uint32)]
 
 
 class _MeshSourceC(ctypes.Structure):
@@ -244,6 +254,15 @@ def load_library() -> ctypes.CDLL:
     lib.mb2_object_manager_host_assets.restype = None
     lib.mb2_object_manager_destroy.argtypes = [vp]
     lib.mb2_object_manager_destroy.restype = None
+    lib.mb2_navmesh_create.argtypes = [vp, ctypes.c_uint32, vp, ctypes.c_uint32, vp, vp, ctypes.c_uint32,
+                                       ctypes.c_int]
+    lib.mb2_navmesh_create.restype = vp
+    lib.mb2_navmesh_view.argtypes = [vp]
+    lib.mb2_navmesh_view.restype = vp
+    lib.mb2_navmesh_host_arrays.argtypes = [vp, ctypes.POINTER(_NavmeshArraysC)]
+    lib.mb2_navmesh_host_arrays.restype = None
+    lib.mb2_navmesh_destroy.argtypes = [vp]
+    lib.mb2_navmesh_destroy.restype = None
     lib.mb2_render_debug_hits.argtypes = [vp]
     lib.mb2_render_debug_hits.restype = vp
     lib.mb2_render_debug_buffer.argtypes = [vp, ctypes.c_int, ctypes.POINTER(ctypes.c_int64)]
@@ -709,6 +728,83 @@ class RigidBodyAssets:
     def close(self):
         if self._h:
             self._lib.mb2_object_manager_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Navmesh:
+    """Host navmesh builder (the reference's host Navmesh::initFromPolygons, include/madrona/
+    navmesh.hpp) for a mesh that many worlds share: the four arrays of a madrona::Navmesh,
+    bit-identical to the reference's, built once and uploaded once to `gpu_id`
+    (gpu_id < 0: host arrays only).
+
+    vertices: [nv, 3] float32; polygons: a list of vertex-index loops (CCW, at least 3
+    each; fanned from the first index) or a pair (flat indices, sizes) with the offsets
+    implied, or a triple (flat indices, offsets, sizes).
+    `view_bytes()` is the 40-byte madrona::Navmesh holding device pointers, to copy into a
+    simulator's Config.  Executors adopt those pointers without owning them: close() the
+    navmesh only after every executor that uses it."""
+
+    def __init__(self, vertices, polygons, gpu_id: int = -1):
+        import numpy as np
+        self._lib = load_library()
+        self._h = None
+        verts = np.ascontiguousarray(vertices, dtype=np.float32).reshape(-1, 3)
+        if isinstance(polygons, tuple) and len(polygons) == 3:
+            idx, offsets, sizes = (np.ascontiguousarray(a, dtype=np.uint32) for a in polygons)
+        elif isinstance(polygons, tuple) and len(polygons) == 2:
+            idx, sizes = (np.ascontiguousarray(a, dtype=np.uint32) for a in polygons)
+            offsets = np.concatenate([[0], np.cumsum(sizes)[:-1]]).astype(np.uint32) if len(sizes) else sizes
+        else:
+            sizes = np.asarray([len(p) for p in polygons], dtype=np.uint32)
+            idx = np.asarray([v for p in polygons for v in p], dtype=np.uint32)
+            offsets = np.concatenate([[0], np.cumsum(sizes)[:-1]]).astype(np.uint32) if len(sizes) else sizes
+        if len(offsets) != len(sizes):
+            raise MadronaB200Error("Navmesh: offsets and sizes differ in length")
+        # keep empty inputs non-null: the builder rejects them with its own message
+        keep = [a if len(a) else np.zeros(1, dtype=a.dtype) for a in (verts.reshape(-1), idx, offsets, sizes)]
+        self._h = self._lib.mb2_navmesh_create(keep[0].ctypes.data, len(verts), keep[1].ctypes.data, len(idx),
+                                               keep[2].ctypes.data, keep[3].ctypes.data, len(sizes), int(gpu_id))
+        if not self._h:
+            raise MadronaB200Error(_last_error(self._lib))
+        self.gpu_id = int(gpu_id)
+
+    def view_bytes(self) -> bytes:
+        """The 40-byte madrona::Navmesh (device pointers, numVerts, numTris)."""
+        p = self._lib.mb2_navmesh_view(self._h)
+        if not p:
+            raise MadronaB200Error("Navmesh was built without a GPU (gpu_id < 0)")
+        return ctypes.string_at(p, 40)
+
+    def arrays(self) -> dict:
+        """Copies of the host arrays: vertices [nv,3] f32, tri_indices and tri_adjacency
+        [T,3] u32, alias_tau [T] f32 and alias [T] u32."""
+        import numpy as np
+        v = _NavmeshArraysC()
+        self._lib.mb2_navmesh_host_arrays(self._h, ctypes.byref(v))
+
+        def arr(ptr, n, dtype):
+            if n == 0:
+                return np.zeros(0, dtype=dtype)
+            raw = ctypes.string_at(ptr, n * np.dtype(dtype).itemsize)
+            return np.frombuffer(raw, dtype=dtype).copy()
+        alias = arr(v.alias_table, 2 * v.num_tris, np.uint32).reshape(-1, 2)
+        return {
+            "vertices": arr(v.vertices, 3 * v.num_verts, np.float32).reshape(-1, 3),
+            "tri_indices": arr(v.tri_indices, 3 * v.num_tris, np.uint32).reshape(-1, 3),
+            "tri_adjacency": arr(v.tri_adjacency, 3 * v.num_tris, np.uint32).reshape(-1, 3),
+            "alias_tau": alias[:, 0].copy().view(np.float32),
+            "alias": alias[:, 1].copy(),
+        }
+
+    def close(self):
+        if self._h:
+            self._lib.mb2_navmesh_destroy(self._h)
             self._h = None
 
     def __del__(self):

@@ -40,6 +40,9 @@ class SimDesc:
     compile_flags: List[str] = field(default_factory=list)
     # batch ray-cast renderer: (cfg) -> (mb2_render_config, keep_alive) or None
     render: Callable = None
+    # (cfg, gpu_id) -> madrona_b200.Navmesh shared by all worlds; its 40-byte view goes
+    # into cfg["_navmesh_view"] for pack_config
+    navmesh: Callable = None
 
 
 def _cartpole_cfg(cfg):
@@ -60,6 +63,18 @@ def _grid_init(w, cfg):
 
 def _customnodes_init(w, cfg):
     return struct.pack("<II", int(cfg.get("seed", 0)) + w, 1 if w % 7 == 3 else 0)
+
+
+def _navmesh_shared(cfg, gpu_id):
+    import madrona_b200 as mb
+    from .navmesh_plan import SHARED_PLAN_SEED, make_plan
+    verts, polys = make_plan(SHARED_PLAN_SEED)
+    return mb.Navmesh(verts, polys, gpu_id)
+
+
+def _navmesh_cfg(cfg):
+    flags = (1 if cfg.get("per_world", True) else 0) | (2 if cfg.get("bad_polygon", False) else 0)
+    return bytes(cfg["_navmesh_view"]) + struct.pack("<II", int(cfg["episode_len"]), flags)
 
 
 def _room_cfg(cfg):
@@ -449,6 +464,27 @@ SIMS: Dict[str, SimDesc] = {
         defaults={"count": 1, "threads": 1, "dynamic": 0, "extra_node_datas": 0, "seed": 0},
         compile_flags=["-DCUSTOMNODES_PROBE=1"],
     ),
+    # navigation meshes: a navmesh per world built in the world constructor and one shared
+    # through Config; agents walk Dijkstra fields towards sampled goals and count what a
+    # predicated BFS reaches (tests/test_navmesh.py).  per_world=False: every agent walks the
+    # shared mesh; bad_polygon=True: world 1's plan has a 2-vertex polygon
+    "navmesh": SimDesc(
+        name="navmesh",
+        sources=[os.path.join(_ROOT, "navmesh", "sim.cpp")],
+        num_exports=7,
+        num_taskgraphs=1,
+        inputs=[],
+        outputs=[Slot(0, "pos", "float32", (6, 3)), Slot(1, "poly", "uint32", (6,)),
+                 Slot(2, "dist", "float32", (6,)), Slot(3, "dijkstra", "uint32", (6, 2)),
+                 Slot(4, "bfs", "uint32", (6, 2)), Slot(5, "goal", "uint32", (6, 4)),
+                 Slot(6, "mesh", "uint32", (6,))],
+        pack_config=_navmesh_cfg,
+        pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
+        oracle_extra=lambda cfg: [int(cfg["episode_len"]), int(cfg.get("seed", 0)),
+                                  1 if cfg.get("per_world", True) else 0],
+        defaults={"episode_len": 40, "seed": 0, "per_world": True, "bad_polygon": False},
+        navmesh=_navmesh_shared,
+    ),
     "cartpole": SimDesc(
         name="cartpole",
         sources=[os.path.join(_ROOT, "cartpole", "sim.cpp")],
@@ -500,6 +536,10 @@ def make_executor(name: str, num_worlds: int, gpu_id: int = 0, objects_fn=None, 
         torch.cuda.synchronize(gpu_id)
         full["obj_mgr_ptr"] = base
         keep_alive = dev_buf
+    navmesh = None
+    if desc.navmesh is not None:
+        navmesh = desc.navmesh(full, gpu_id)
+        full["_navmesh_view"] = navmesh.view_bytes()
     inits = pack_world_inits(desc, num_worlds, full)
     state = mb.StateConfig(
         worldInit=inits,
@@ -517,5 +557,5 @@ def make_executor(name: str, num_worlds: int, gpu_id: int = 0, objects_fn=None, 
     full["_gpu_id"] = gpu_id
     render_cfg, render_keep = (desc.render(full) if desc.render is not None else (None, None))
     ex = mb.MWCudaExecutor(state, compile_cfg, gpu_id=gpu_id, render_cfg=render_cfg)
-    ex._keep_alive = (keep_alive, render_keep)
+    ex._keep_alive = (keep_alive, render_keep, navmesh)
     return ex
