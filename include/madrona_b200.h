@@ -78,14 +78,23 @@ typedef struct mb2_material_view {
 } mb2_material_view;
 
 /* == madrona::CudaBatchRenderConfig, include/madrona/mw_gpu.hpp:75-96 (same
- * fields, same order). */
+ * fields, same order), then the image size.  Each view's output is row-major
+ * [render_height][render_width]: RGBA8 plus f32 depth (RGBD) or depth only.
+ * Both 0 (what a caller that fills only the first six fields passes when it
+ * zero-initialises the struct): a render_resolution square.  Set together; a
+ * nonzero render_resolution must then equal both.  The vertical field of view
+ * spans the rows, the horizontal one is widened by width / height.
+ * render_width * render_height * 4 must fit in 32 bits.  mb2_executor_create
+ * returns NULL and mb2_last_error() says why when any of this does not hold. */
 typedef struct mb2_render_config {
     uint32_t render_mode;          /* 0 RGBD, 1 Depth */
     mb2_mesh_bvh_view geo_bvh_data;
     mb2_material_view material_data;
-    uint32_t render_resolution;    /* square output */
+    uint32_t render_resolution;    /* square output, unless render_width / render_height are set */
     float near_plane;
     float far_plane;
+    uint32_t render_width;         /* columns per view, or 0 */
+    uint32_t render_height;        /* rows per view, or 0 */
 } mb2_render_config;
 
 /* Triangle mesh -> BLAS.  Role of MeshBVHBuilder (src/common/mesh_bvh_builder.cpp,

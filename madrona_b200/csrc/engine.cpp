@@ -360,6 +360,15 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
         setError("too many exported buffers");
         return false;
     }
+    if (rc) {
+        // the image size is checked before any CUDA call or allocation
+        uint32_t width, height;
+        std::string err;
+        if (!renderImageSize(rc, &width, &height, &err)) {
+            setError(err);
+            return false;
+        }
+    }
 
     MB2_CUDA(cudaSetDevice(ex->gpu));
     cudaDeviceProp prop;

@@ -15,6 +15,8 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
                          std::string *err);
 LaunchGraph *physicsBuildRenderGraph(Executor *ex, std::string *err);
 // batch ray-cast renderer (kernels_render.cu)
+// the image size of a render config, or false and why the config is invalid
+bool renderImageSize(const mb2_render_config *rc, uint32_t *width, uint32_t *height, std::string *err);
 bool renderHostCreate(Executor *ex, const mb2_render_config *rc, std::string *err);
 bool renderHostAfterRegistry(Executor *ex, std::string *err);
 void renderHostDestroy(Executor *ex);

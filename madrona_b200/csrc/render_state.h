@@ -77,8 +77,8 @@ struct ViewArchetype {
 struct RenderState {
     // ---- host config (before registerTypes)
     u32 enabled;
-    u32 resolution;
-    u32 rgbd;              // 1 = RGB + depth, 0 = depth only
+    u32 width, height;     // image size of every view: [height][width] pixels, row-major
+    u32 rgbd;            // 1 = RGB + depth, 0 = depth only
     float nearPlane, farPlane;
     const MeshBVH *meshes;          // device, == CudaBatchRenderConfig::geoBVHData.meshBVHs
     u32 numMeshes;
@@ -121,7 +121,7 @@ struct RenderState {
     i32 lightCol;
     RenderView *views;              // [capacity of the output archetype]
     i32 maxViews;
-    i32 *hitIDs;                    // debug: [maxViews][res*res][2] = (instance, triangle) or -1
+    i32 *hitIDs;                    // debug: [maxViews][height*width][2] = (instance, triangle) or -1
     // exportCountsGPU (src/render/ecs_system.cpp:317-348): totals of the last prepare
     u32 totalNumViews;
     u32 totalNumInstances;

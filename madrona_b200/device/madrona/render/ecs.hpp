@@ -98,9 +98,10 @@ inline void registerTypes(ECSRegistry &registry, const RenderECSBridge *)
     registry.registerComponent<LightDescActive>();
     registry.registerComponent<LightCarrier>();
 
-    // one output row per view: res x res RGBA8 and res x res f32 depth
-    // (src/render/ecs_system.cpp: registerComponent<...OutputBuffer>(bytes))
-    uint32_t pixels = R.resolution * R.resolution;
+    // one output row per view: height x width RGBA8 and height x width f32 depth
+    // (src/render/ecs_system.cpp: registerComponent<...OutputBuffer>(bytes));
+    // renderHostCreate rejects sizes whose bytes do not fit 32 bits
+    uint32_t pixels = R.width * R.height;
     uint32_t bytes = pixels * 4u;
     if (bytes == 0) bytes = 4;
     registry.registerComponent<RGBOutputBuffer>(bytes);

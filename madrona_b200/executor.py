@@ -110,7 +110,7 @@ class _MaterialViewC(ctypes.Structure):      # == render::MaterialData
     ]
 
 
-class _RenderConfigC(ctypes.Structure):      # == madrona::CudaBatchRenderConfig
+class _RenderConfigC(ctypes.Structure):      # == madrona::CudaBatchRenderConfig + image size
     _fields_ = [
         ("render_mode", ctypes.c_uint32),
         ("geo_bvh_data", _MeshBVHViewC),
@@ -118,6 +118,9 @@ class _RenderConfigC(ctypes.Structure):      # == madrona::CudaBatchRenderConfig
         ("render_resolution", ctypes.c_uint32),
         ("near_plane", ctypes.c_float),
         ("far_plane", ctypes.c_float),
+        # non-square images: both nonzero, render_resolution 0 (or equal to both)
+        ("render_width", ctypes.c_uint32),
+        ("render_height", ctypes.c_uint32),
     ]
 
 
@@ -482,13 +485,14 @@ class MWCudaExecutor:
         from .tensor import Tensor
         return Tensor(self.getExported(slot), type, dimensions, gpu_id=self.gpu_id)
 
-    def renderDebugHits(self, num_views: int, resolution: int):
-        """int32 [views, res, res, 2] (instance, triangle) per pixel; needs MADRONA_B200_RENDER_DEBUG=1."""
+    def renderDebugHits(self, num_views: int, height: int, width: Optional[int] = None):
+        """int32 [views, height, width, 2] (instance, triangle) per pixel; width defaults to height
+        (square images).  Needs MADRONA_B200_RENDER_DEBUG=1."""
         import torch
         p = self._lib.mb2_render_debug_hits(self._h)
         if not p:
             raise MadronaB200Error("no debug hit buffer (set MADRONA_B200_RENDER_DEBUG=1 before creating the executor)")
-        view = _CudaView(p, (num_views, resolution, resolution, 2), "<i4")
+        view = _CudaView(p, (num_views, height, height if width is None else width, 2), "<i4")
         return torch.as_tensor(view, device=f"cuda:{self.gpu_id}")
 
     def renderDebugStructures(self):

@@ -138,6 +138,20 @@ struct CudaBatchRenderConfig {
     float farPlane = 0.f;
 };
 
+}
+
+namespace madrona_b200 {
+// Image size of every view for the MWCudaExecutor constructor overload that takes one:
+// row-major [height][width] pixels, the vertical field of view spanning the rows.  Given
+// with a CudaBatchRenderConfig whose renderResolution is 0 (or equal to both).
+struct RenderImageSize {
+    uint32_t width;
+    uint32_t height;
+};
+}
+
+namespace madrona {
+
 namespace detail {
 [[noreturn]] inline void fatal(const char *what)
 {
@@ -188,33 +202,16 @@ public:
                    const Optional<CudaBatchRenderConfig> &render_cfg =
                        Optional<CudaBatchRenderConfig>::none())
     {
-        mb2_state_config sc {
-            state_cfg.worldInitPtr, state_cfg.numWorldInitBytes,
-            state_cfg.userConfigPtr, state_cfg.numUserConfigBytes,
-            state_cfg.numWorldDataBytes, state_cfg.worldDataAlignment,
-            state_cfg.numWorlds, state_cfg.numTaskGraphs, state_cfg.numExportedBuffers,
-        };
-        mb2_compile_config cc {
-            compile_cfg.userSources.data(), (uint32_t)compile_cfg.userSources.size(),
-            compile_cfg.userCompileFlags.data(), (uint32_t)compile_cfg.userCompileFlags.size(),
-            (uint32_t)compile_cfg.optMode,
-        };
-        mb2_render_config rc {};
-        if (render_cfg.has_value()) {
-            static_assert(sizeof(render::MeshBVHData) == sizeof(mb2_mesh_bvh_view), "MeshBVHData layout");
-            rc.render_mode = (uint32_t)render_cfg->renderMode;
-            memcpy(&rc.geo_bvh_data, &render_cfg->geoBVHData, sizeof(rc.geo_bvh_data));
-            rc.material_data.textures = (void *)render_cfg->materialData.textures;
-            rc.material_data.num_texture_buffers = render_cfg->materialData.numTextureBuffers;
-            rc.material_data.texture_buffers = (void *)render_cfg->materialData.textureBuffers;
-            rc.material_data.materials = (void *)render_cfg->materialData.materials;
-            rc.render_resolution = render_cfg->renderResolution;
-            rc.near_plane = render_cfg->nearPlane;
-            rc.far_plane = render_cfg->farPlane;
-        }
-        int gpu_id = mb2_device_of_context((void *)cu_ctx);
-        h_ = mb2_executor_create(&sc, &cc, gpu_id, render_cfg.has_value() ? &rc : nullptr);
-        if (!h_) detail::fatal("MWCudaExecutor");
+        create(state_cfg, compile_cfg, cu_ctx, render_cfg, ::madrona_b200::RenderImageSize { 0, 0 });
+    }
+
+    // Not in the reference: the batch renderer's images are image_size.width columns by
+    // image_size.height rows instead of renderResolution squared.
+    MWCudaExecutor(const StateConfig &state_cfg, const CompileConfig &compile_cfg,
+                   CUcontext cu_ctx, const Optional<CudaBatchRenderConfig> &render_cfg,
+                   const ::madrona_b200::RenderImageSize &image_size)
+    {
+        create(state_cfg, compile_cfg, cu_ctx, render_cfg, image_size);
     }
 
     MWCudaExecutor(MWCudaExecutor &&o) : h_(o.h_) { o.h_ = nullptr; }
@@ -276,6 +273,41 @@ public:
     void *getExported(CountT slot) const { return mb2_get_exported(h_, (int64_t)slot); }
 
 private:
+    void create(const StateConfig &state_cfg, const CompileConfig &compile_cfg, CUcontext cu_ctx,
+                const Optional<CudaBatchRenderConfig> &render_cfg,
+                const ::madrona_b200::RenderImageSize &image_size)
+    {
+        mb2_state_config sc {
+            state_cfg.worldInitPtr, state_cfg.numWorldInitBytes,
+            state_cfg.userConfigPtr, state_cfg.numUserConfigBytes,
+            state_cfg.numWorldDataBytes, state_cfg.worldDataAlignment,
+            state_cfg.numWorlds, state_cfg.numTaskGraphs, state_cfg.numExportedBuffers,
+        };
+        mb2_compile_config cc {
+            compile_cfg.userSources.data(), (uint32_t)compile_cfg.userSources.size(),
+            compile_cfg.userCompileFlags.data(), (uint32_t)compile_cfg.userCompileFlags.size(),
+            (uint32_t)compile_cfg.optMode,
+        };
+        mb2_render_config rc {};
+        if (render_cfg.has_value()) {
+            static_assert(sizeof(render::MeshBVHData) == sizeof(mb2_mesh_bvh_view), "MeshBVHData layout");
+            rc.render_mode = (uint32_t)render_cfg->renderMode;
+            memcpy(&rc.geo_bvh_data, &render_cfg->geoBVHData, sizeof(rc.geo_bvh_data));
+            rc.material_data.textures = (void *)render_cfg->materialData.textures;
+            rc.material_data.num_texture_buffers = render_cfg->materialData.numTextureBuffers;
+            rc.material_data.texture_buffers = (void *)render_cfg->materialData.textureBuffers;
+            rc.material_data.materials = (void *)render_cfg->materialData.materials;
+            rc.render_resolution = render_cfg->renderResolution;
+            rc.near_plane = render_cfg->nearPlane;
+            rc.far_plane = render_cfg->farPlane;
+            rc.render_width = image_size.width;
+            rc.render_height = image_size.height;
+        }
+        int gpu_id = mb2_device_of_context((void *)cu_ctx);
+        h_ = mb2_executor_create(&sc, &cc, gpu_id, render_cfg.has_value() ? &rc : nullptr);
+        if (!h_) detail::fatal("MWCudaExecutor");
+    }
+
     mb2_executor *h_;
 };
 

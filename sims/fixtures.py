@@ -106,10 +106,19 @@ def _triggers_objects():
     return triggers_objects()
 
 
+def _image_size(cfg, default_res):
+    """Render config image size from the fixture config: keyword arguments for the
+    render_assets builders.  `width` and `height` (both) give non-square images, else the
+    `resolution` square."""
+    if "width" in cfg or "height" in cfg:
+        return {"resolution": 0, "width": int(cfg.get("width", 0)), "height": int(cfg.get("height", 0))}
+    return {"resolution": int(cfg.get("resolution", default_res))}
+
+
 def _room_render_cfg(cfg):
     from .render_assets import make_render_config
-    return make_render_config(int(cfg.get("resolution", 64)), bool(cfg.get("rgbd", False)),
-                              gpu_id=int(cfg.get("_gpu_id", 0)))
+    return make_render_config(rgbd=bool(cfg.get("rgbd", False)), gpu_id=int(cfg.get("_gpu_id", 0)),
+                              **_image_size(cfg, 64))
 
 
 SIMS: Dict[str, SimDesc] = {
@@ -287,7 +296,7 @@ SIMS: Dict[str, SimDesc] = {
         oracle_extra=lambda cfg: [],
         defaults={"num_props": 100, "seed": 0, "resolution": 40, "rgbd": True},
         render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_render_config(
-            int(cfg.get("resolution", 40)), bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0))),
+            rgbd=bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)), **_image_size(cfg, 40)),
     ),
     # GPU only: the gallery built with -DGALLERY_PER_WORLD=1: props[w] props in world w (every
     # 17th hidden, as in the gallery), layouts[w] 0 scattered / 1 clustered (deep Morton tree)
@@ -305,7 +314,7 @@ SIMS: Dict[str, SimDesc] = {
         defaults={"props": [100], "layouts": None, "seed": 0, "resolution": 40, "rgbd": True},
         compile_flags=["-DGALLERY_PER_WORLD=1"],
         render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_render_config(
-            int(cfg.get("resolution", 40)), bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0))),
+            rgbd=bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)), **_image_size(cfg, 40)),
     ),
     # GPU only: the gallery sim with uvs and textured materials (tests/test_render_textures.py);
     # same sources and flags, so it shares the gallery's simulator module
@@ -321,8 +330,8 @@ SIMS: Dict[str, SimDesc] = {
         oracle_extra=lambda cfg: [],
         defaults={"num_props": 100, "seed": 0, "resolution": 40, "rgbd": True, "bc7": False},
         render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_textured_render_config(
-            int(cfg.get("resolution", 40)), bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)),
-            bc7=bool(cfg.get("bc7", False))),
+            rgbd=bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)),
+            bc7=bool(cfg.get("bc7", False)), **_image_size(cfg, 40)),
     ),
     # GPU only: 145 bodies per world, past the per-world body cap (tests/test_cliffs.py)
     "balls_cliff": SimDesc(

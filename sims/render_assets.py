@@ -47,9 +47,11 @@ def mesh_list(descs, verts, indices):
     return out
 
 
-def make_render_config_from_meshes(meshes, resolution: int, rgbd: bool, gpu_id: int = 0, materials=None):
+def make_render_config_from_meshes(meshes, resolution: int, rgbd: bool, gpu_id: int = 0, materials=None,
+                                   width: int = 0, height: int = 0):
     """mb2_render_config (== CudaBatchRenderConfig) whose geoBVHData was built by the
-    engine's BLAS builder; returns (config, keep_alive)."""
+    engine's BLAS builder; returns (config, keep_alive).  width x height images when both are
+    given (resolution then 0 or equal to both), else resolution squared."""
     import madrona_b200 as mb
     from madrona_b200.executor import _MaterialViewC, _RenderConfigC
 
@@ -61,13 +63,15 @@ def make_render_config_from_meshes(meshes, resolution: int, rgbd: bool, gpu_id: 
         m = torch.from_numpy(np.ascontiguousarray(materials, dtype=np.float32)).to(f"cuda:{gpu_id}")
         keep.append(m)
         mat_view = _MaterialViewC(None, 0, None, m.data_ptr())
-    rc = _RenderConfigC(0 if rgbd else 1, bvh.view(device=True), mat_view, resolution, 0.001, 1000.0)
+    rc = _RenderConfigC(0 if rgbd else 1, bvh.view(device=True), mat_view, resolution, 0.001, 1000.0,
+                        width, height)
     return rc, keep
 
 
-def make_render_config(resolution: int, rgbd: bool = False, gpu_id: int = 0):
+def make_render_config(resolution: int, rgbd: bool = False, gpu_id: int = 0, width: int = 0, height: int = 0):
     descs, verts, indices = room_meshes()
-    return make_render_config_from_meshes(mesh_list(descs, verts, indices), resolution, rgbd, gpu_id)
+    return make_render_config_from_meshes(mesh_list(descs, verts, indices), resolution, rgbd, gpu_id,
+                                          width=width, height=height)
 
 
 # ---- gallery fixture: four prop meshes + ground ------------------------------------------------
@@ -133,8 +137,9 @@ GALLERY_MATERIALS = np.array([
 GALLERY_MATERIALS[:, 4] = np.array([-1], dtype=np.int32).view(np.float32)[0]     # textureIdx = -1
 
 
-def make_gallery_render_config(resolution: int, rgbd: bool, gpu_id: int = 0):
-    return make_render_config_from_meshes(gallery_meshes(), resolution, rgbd, gpu_id, materials=GALLERY_MATERIALS)
+def make_gallery_render_config(resolution: int, rgbd: bool, gpu_id: int = 0, width: int = 0, height: int = 0):
+    return make_render_config_from_meshes(gallery_meshes(), resolution, rgbd, gpu_id, materials=GALLERY_MATERIALS,
+                                          width=width, height=height)
 
 
 # ---- textured gallery: the same meshes with uvs, three generated textures -----------------------
@@ -281,7 +286,8 @@ def gallery_textured_materials(bc7: bool = False):
             for i, m in enumerate(GALLERY_MATERIALS)]
 
 
-def make_gallery_textured_render_config(resolution: int, rgbd: bool, gpu_id: int = 0, bc7: bool = False):
+def make_gallery_textured_render_config(resolution: int, rgbd: bool, gpu_id: int = 0, bc7: bool = False,
+                                        width: int = 0, height: int = 0):
     """CudaBatchRenderConfig with textured materials uploaded by mb2_init_material_data; the
     MaterialData in keep_alive must outlive the executor."""
     import madrona_b200 as mb
@@ -290,5 +296,6 @@ def make_gallery_textured_render_config(resolution: int, rgbd: bool, gpu_id: int
     bvh = mb.MeshBVHData(gallery_textured_meshes(), gpu_id=gpu_id)
     textures = [(src, fmt, t.shape[1], t.shape[0]) for t, fmt, src in gallery_textures()]
     mats = mb.MaterialData(gallery_textured_materials(bc7), textures, gpu_id=gpu_id)
-    rc = _RenderConfigC(0 if rgbd else 1, bvh.view(device=True), mats.view(), resolution, 0.001, 1000.0)
+    rc = _RenderConfigC(0 if rgbd else 1, bvh.view(device=True), mats.view(), resolution, 0.001, 1000.0,
+                        width, height)
     return rc, [bvh, mats]
