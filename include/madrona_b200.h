@@ -374,6 +374,35 @@ int mb2_peer_gather_release_async(mb2_peer_gather *gather, void *cuda_stream);
 void *mb2_peer_gather_buffer(mb2_peer_gather *gather, uint32_t parity, uint32_t slot_index);
 void mb2_peer_gather_destroy(mb2_peer_gather *gather);
 
+/* ---- snapshots of an executor's simulation state ----------------------------
+ * No reference counterpart.  A snapshot is a device buffer that holds every
+ * byte of device state a later launch graph can read: the live rows of every
+ * table, the entity store, world data, the persistent and tmp arenas, custom
+ * node data and the ray caster's last prepared scene.  save copies the live
+ * state into it, restore copies it back; each is one kernel launch on
+ * cuda_stream (NULL: the legacy default stream), ordered like run_async and
+ * never synchronizing the host.  Stepping after a restore reproduces, bit for
+ * bit, what stepping after the save did.
+ *   - a snapshot belongs to the executor that created it: save / restore with
+ *     another executor, restore before any save, and null handles fail with a
+ *     message in mb2_last_error() (return 1) and launch nothing;
+ *   - it is sized for the table capacities at creation; a save after a table
+ *     grew enlarges it first (stream-ordered), a restore always fits;
+ *   - it shares the executor's tables, so it is part of the "one launch graph
+ *     in flight" rule: order saves and restores with the executor's launches;
+ *   - destroy snapshots before their executor; destroy waits for the device.
+ * mb2_snapshot_bytes is the size of the buffer, which holds every table and
+ * arena at its capacity; mb2_snapshot_saved_bytes is what the last save
+ * copied, the live part (0 before a save; it waits for the device).  Both
+ * return -1 for a null handle. */
+typedef struct mb2_snapshot mb2_snapshot;
+mb2_snapshot *mb2_snapshot_create(mb2_executor *exec);
+int mb2_snapshot_save(mb2_executor *exec, mb2_snapshot *snap, void *cuda_stream);
+int mb2_snapshot_restore(mb2_executor *exec, mb2_snapshot *snap, void *cuda_stream);
+int64_t mb2_snapshot_bytes(const mb2_snapshot *snap);
+int64_t mb2_snapshot_saved_bytes(mb2_snapshot *snap);
+void mb2_snapshot_destroy(mb2_snapshot *snap);
+
 /* Version string. */
 const char *mb2_version(void);
 

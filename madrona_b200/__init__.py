@@ -21,6 +21,7 @@ from .executor import (  # noqa: F401
     RigidBodyAssets,
     Navmesh,
     PeerGather,
+    Snapshot,
 )
 from .tensor import (  # noqa: F401
     Tensor, TensorElementType, NamedTensor, TrainInterface, TrainStepInputInterface,

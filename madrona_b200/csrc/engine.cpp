@@ -1287,6 +1287,65 @@ void *mb2_executor_stream(mb2_executor *exec)
     return exec ? (void *)((Executor *)exec)->stream : nullptr;
 }
 
+mb2_snapshot *mb2_snapshot_create(mb2_executor *exec)
+{
+    g_last_error.clear();
+    if (!exec) {
+        setError("mb2_snapshot_create: null executor");
+        return nullptr;
+    }
+    std::string err;
+    Snapshot *s = snapshotCreate((Executor *)exec, &err);
+    if (!s) setError(err);
+    return (mb2_snapshot *)s;
+}
+
+// save / restore: the same checks, then one launch
+static int snapshotCall(mb2_executor *exec, mb2_snapshot *snap, void *cuda_stream, bool restore)
+{
+    g_last_error.clear();
+    const char *what = restore ? "mb2_snapshot_restore" : "mb2_snapshot_save";
+    if (!exec || !snap) {
+        setError(std::string(what) + ": null executor or snapshot");
+        return 1;
+    }
+    Snapshot *s = (Snapshot *)snap;
+    if (snapshotOwner(s) != (Executor *)exec) {
+        setError(std::string(what) + ": the snapshot belongs to another executor");
+        return 1;
+    }
+    std::string err;
+    const bool ok = restore ? snapshotRestore(s, (cudaStream_t)cuda_stream, &err)
+                            : snapshotSave(s, (cudaStream_t)cuda_stream, &err);
+    if (!ok) {
+        setError(err);
+        return 1;
+    }
+    return 0;
+}
+
+int mb2_snapshot_save(mb2_executor *exec, mb2_snapshot *snap, void *cuda_stream)
+{
+    return snapshotCall(exec, snap, cuda_stream, false);
+}
+
+int mb2_snapshot_restore(mb2_executor *exec, mb2_snapshot *snap, void *cuda_stream)
+{
+    return snapshotCall(exec, snap, cuda_stream, true);
+}
+
+int64_t mb2_snapshot_bytes(const mb2_snapshot *snap)
+{
+    return snap ? snapshotBytes((const Snapshot *)snap) : -1;
+}
+
+int64_t mb2_snapshot_saved_bytes(mb2_snapshot *snap)
+{
+    return snap ? snapshotSavedBytes((Snapshot *)snap) : -1;
+}
+
+void mb2_snapshot_destroy(mb2_snapshot *snap) { snapshotDestroy((Snapshot *)snap); }
+
 int mb2_jit_precompile(const mb2_compile_config *cc)
 {
     g_last_error.clear();

@@ -86,4 +86,15 @@ bool sortScratchEnsure(Executor *ex, int32_t max_rows, std::string *err);
 // grow a dynamic table to new_capacity rows (columns, twins, entity store, sort scratch)
 bool growTable(Executor *ex, uint32_t archetype, int64_t new_capacity, std::string *err);
 
+// ---- snapshots of the device state (kernels_snapshot.cu) -----------------------------
+struct Snapshot;
+Snapshot *snapshotCreate(Executor *ex, std::string *err);
+// one launch on `s` each; save first enlarges the snapshot if a table grew since
+bool snapshotSave(Snapshot *snap, cudaStream_t s, std::string *err);
+bool snapshotRestore(Snapshot *snap, cudaStream_t s, std::string *err);
+int64_t snapshotBytes(const Snapshot *snap);
+int64_t snapshotSavedBytes(Snapshot *snap);
+Executor *snapshotOwner(const Snapshot *snap);
+void snapshotDestroy(Snapshot *snap);
+
 }

@@ -1843,6 +1843,12 @@ void *renderDebugHitBuffer(Executor *ex)
     return (rh && rh->active) ? (void *)rh->hRender.hitIDs : nullptr;
 }
 
+const RenderState *renderHostState(Executor *ex)
+{
+    RenderHost *rh = ex->render;
+    return (rh && rh->active) ? &rh->hRender : nullptr;
+}
+
 void *renderDebugBuffer(Executor *ex, int which)
 {
     RenderHost *rh = ex->render;

@@ -26,6 +26,8 @@ bool renderEnsureCapacity(Executor *ex, std::string *err);
 void *renderDebugHitBuffer(Executor *ex);
 void *renderDebugBuffer(Executor *ex, int which);
 uint64_t renderBytesPerFrame(Executor *ex, int64_t num_views);
+// host copy of the ray caster's state (device pointers, capacities), null when it is not active
+const RenderState *renderHostState(Executor *ex);
 // algorithmic bytes of one launch of a physics node + a short name (profiling)
 uint64_t physicsNodeBytes(Executor *ex, const NodeRecord &rec, const char **name, int64_t *rows);
 

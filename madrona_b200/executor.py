@@ -10,6 +10,7 @@ from __future__ import annotations
 
 import ctypes
 import os
+import weakref
 from dataclasses import dataclass, field
 from typing import Optional, Sequence
 
@@ -63,6 +64,12 @@ EXPORTED_SYMBOLS = [
     "mb2_peer_gather_release_async",
     "mb2_peer_gather_buffer",
     "mb2_peer_gather_destroy",
+    "mb2_snapshot_create",
+    "mb2_snapshot_save",
+    "mb2_snapshot_restore",
+    "mb2_snapshot_bytes",
+    "mb2_snapshot_saved_bytes",
+    "mb2_snapshot_destroy",
 ]
 
 
@@ -285,6 +292,18 @@ def load_library() -> ctypes.CDLL:
     lib.mb2_peer_gather_buffer.restype = vp
     lib.mb2_peer_gather_destroy.argtypes = [vp]
     lib.mb2_peer_gather_destroy.restype = None
+    lib.mb2_snapshot_create.argtypes = [vp]
+    lib.mb2_snapshot_create.restype = vp
+    for name in ("save", "restore"):
+        fn = getattr(lib, f"mb2_snapshot_{name}")
+        fn.argtypes = [vp, vp, vp]
+        fn.restype = ctypes.c_int
+    lib.mb2_snapshot_bytes.argtypes = [vp]
+    lib.mb2_snapshot_bytes.restype = ctypes.c_int64
+    lib.mb2_snapshot_saved_bytes.argtypes = [vp]
+    lib.mb2_snapshot_saved_bytes.restype = ctypes.c_int64
+    lib.mb2_snapshot_destroy.argtypes = [vp]
+    lib.mb2_snapshot_destroy.restype = None
     _LIB = lib
     return lib
 
@@ -391,6 +410,7 @@ class MWCudaExecutor:
                  gpu_id: int = 0, render_cfg=None):
         self._lib = load_library()
         self._h = None
+        self._snapshots = weakref.WeakSet()
         self.gpu_id = gpu_id
         self.num_worlds = state_cfg.numWorlds
         self.num_taskgraphs = state_cfg.numTaskGraphs
@@ -522,10 +542,78 @@ class MWCudaExecutor:
         this rank's columns; returns a PeerGather whose handle must be exchanged."""
         return PeerGather(self, slots, shapes, dtypes, world_size, rank)
 
+    def snapshot(self) -> "Snapshot":
+        """A device-memory snapshot of this executor's simulation state, empty until its
+        first save() (include/madrona_b200.h)."""
+        return Snapshot(self)
+
     def close(self) -> None:
         if self._h:
+            # snapshots go before their executor
+            for snap in list(getattr(self, "_snapshots", ())):
+                snap.close()
             self._lib.mb2_executor_destroy(self._h)
             self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Snapshot:
+    """Every byte of an executor's device state that a later step can read, held in device
+    memory: save() copies the live state in, restore() copies it back, each one kernel launch
+    on `stream` (None: the executor's stream; a torch.cuda.Stream or a raw handle as runAsync
+    takes it) without synchronizing the host.  Stepping after restore() reproduces what
+    stepping after save() did, bit for bit.  Only the executor that made the snapshot can
+    restore it; exported tensors keep their addresses and see the restored rows."""
+
+    def __init__(self, ex: "MWCudaExecutor"):
+        self._lib = ex._lib
+        self._ex = ex
+        self._h = None
+        h = self._lib.mb2_snapshot_create(ex._h)
+        if not h:
+            raise MadronaB200Error(_last_error(self._lib))
+        self._h = h
+        ex._snapshots.add(self)
+
+    def _call(self, name, stream):
+        if not self._h:
+            raise MadronaB200Error(f"snapshot {name}: the snapshot is closed")
+        s = self._ex.stream if stream is None else int(getattr(stream, "cuda_stream", stream))
+        if getattr(self._lib, f"mb2_snapshot_{name}")(self._ex._h, self._h, ctypes.c_void_p(s)) != 0:
+            raise MadronaB200Error(_last_error(self._lib))
+
+    def save(self, stream=None) -> None:
+        self._call("save", stream)
+
+    def restore(self, stream=None) -> None:
+        self._call("restore", stream)
+
+    @property
+    def nbytes(self) -> int:
+        """Bytes of device memory the snapshot holds (it grows when a save follows table growth)."""
+        return int(self._lib.mb2_snapshot_bytes(self._h)) if self._h else 0
+
+    @property
+    def saved_nbytes(self) -> int:
+        """Bytes the last save() copied: the live part of the state (waits for the device)."""
+        return int(self._lib.mb2_snapshot_saved_bytes(self._h)) if self._h else 0
+
+    def close(self) -> None:
+        if self._h:
+            if self._ex._h:
+                self._lib.mb2_snapshot_destroy(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
     def __del__(self):
         try:

@@ -140,6 +140,8 @@ struct CudaBatchRenderConfig {
 
 }
 
+namespace madrona { class MWCudaExecutor; }
+
 namespace madrona_b200 {
 // Image size of every view for the MWCudaExecutor constructor overload that takes one:
 // row-major [height][width] pixels, the vertical field of view spanning the rows.  Given
@@ -147,6 +149,40 @@ namespace madrona_b200 {
 struct RenderImageSize {
     uint32_t width;
     uint32_t height;
+};
+
+// A device-memory snapshot of an executor's simulation state (include/madrona_b200.h),
+// made by MWCudaExecutor::snapshot().  save() / restore() are one kernel launch each on
+// `strm` (by default the executor's stream) and never synchronize the host; stepping after
+// restore() reproduces what stepping after save() did.  Destroy it before its executor.
+class ExecutorSnapshot {
+public:
+    ExecutorSnapshot() : exec_(nullptr), h_(nullptr) {}
+    ExecutorSnapshot(ExecutorSnapshot &&o) : exec_(o.exec_), h_(o.h_) { o.h_ = nullptr; }
+    ~ExecutorSnapshot() { if (h_) mb2_snapshot_destroy(h_); }
+    ExecutorSnapshot &operator=(ExecutorSnapshot &&o)
+    {
+        if (this != &o) {
+            if (h_) mb2_snapshot_destroy(h_);
+            exec_ = o.exec_;
+            h_ = o.h_;
+            o.h_ = nullptr;
+        }
+        return *this;
+    }
+
+    inline void save(cudaStream_t strm);
+    inline void restore(cudaStream_t strm);
+    void save() { save((cudaStream_t)mb2_executor_stream(exec_)); }
+    void restore() { restore((cudaStream_t)mb2_executor_stream(exec_)); }
+    // bytes of device memory the snapshot holds
+    int64_t bytes() const { return mb2_snapshot_bytes(h_); }
+
+private:
+    ExecutorSnapshot(mb2_executor *exec, mb2_snapshot *h) : exec_(exec), h_(h) {}
+    mb2_executor *exec_;
+    mb2_snapshot *h_;
+friend class ::madrona::MWCudaExecutor;
 };
 }
 
@@ -272,6 +308,14 @@ public:
 
     void *getExported(CountT slot) const { return mb2_get_exported(h_, (int64_t)slot); }
 
+    // Not in the reference: a snapshot of this executor's state (empty until its first save)
+    ::madrona_b200::ExecutorSnapshot snapshot()
+    {
+        mb2_snapshot *s = mb2_snapshot_create(h_);
+        if (!s) detail::fatal("snapshot");
+        return ::madrona_b200::ExecutorSnapshot(h_, s);
+    }
+
 private:
     void create(const StateConfig &state_cfg, const CompileConfig &compile_cfg, CUcontext cu_ctx,
                 const Optional<CudaBatchRenderConfig> &render_cfg,
@@ -311,4 +355,14 @@ private:
     mb2_executor *h_;
 };
 
+}
+
+inline void madrona_b200::ExecutorSnapshot::save(cudaStream_t strm)
+{
+    if (mb2_snapshot_save(exec_, h_, (void *)strm) != 0) ::madrona::detail::fatal("ExecutorSnapshot::save");
+}
+
+inline void madrona_b200::ExecutorSnapshot::restore(cudaStream_t strm)
+{
+    if (mb2_snapshot_restore(exec_, h_, (void *)strm) != 0) ::madrona::detail::fatal("ExecutorSnapshot::restore");
 }
