@@ -873,8 +873,10 @@ __device__ __forceinline__ bool gaussMapArcsCross(Vector3 a, Vector3 b, Vector3 
     return cba * dba < 0.0f && adc * bdc < 0.0f && cba * bdc > 0.0f;
 }
 
-// Sutherland-Hodgman against one plane; "<= 0" is inside (narrowphase.cpp:617-652)
-__device__ __forceinline__ int clipAgainst(Vector3 *dst, const Plane &pl, const Vector3 *src, int n)
+// Sutherland-Hodgman against one plane; "<= 0" is inside (narrowphase.cpp:617-652).
+// dst holds `cap` points: returns -1, having written nothing past dst[cap - 1], when
+// the clipped polygon would not fit.
+__device__ __forceinline__ int clipAgainst(Vector3 *dst, const Plane &pl, const Vector3 *src, int n, int cap)
 {
     int m = 0;
     Vector3 v1 = src[n - 1];
@@ -884,10 +886,13 @@ __device__ __forceinline__ int clipAgainst(Vector3 *dst, const Plane &pl, const 
         Vector3 v2 = src[i];
         float d2 = planeDistance(pl, v2);
         if (d1 <= 0.0f && d2 <= 0.0f) {
+            if (m == cap) return -1;
             dst[m++] = v2;
         } else if (d1 <= 0.0f && d2 > 0.0f) {
+            if (m == cap) return -1;
             dst[m++] = v1 + (v2 - v1) * (-d1 / pl.normal.dot(v2 - v1));
         } else if (d2 <= 0.0f && d1 > 0.0f) {
+            if (m + 2 > cap) return -1;
             dst[m++] = v1 + (v2 - v1) * (-d1 / pl.normal.dot(v2 - v1));
             dst[m++] = v2;
         }
@@ -1537,7 +1542,9 @@ __device__ bool hullHullGroup(EngineState &S, const PairSetup &ps, HullScratch &
     if (inc_face == 0x7fffffff) return false;
 
     // incident polygon clipped against the side planes of the reference face
-    // (normal = edge x n_ref), on the group's first lane; result in clipA (0) or clipB (1)
+    // (normal = edge x n_ref), on the group's first lane; result in clipA (0) or clipB (1).
+    // Either face over kMaxFaceVerts vertices, or a clipped polygon over kClipCap points
+    // (k-gon against k-gon: up to 2k), is an overflow: n = -1, and no contact.
     int n = 0, in_b = 0;
     if (sub == 0) {
         Vector3 *src = scratch.clipA, *dst = scratch.clipB;
@@ -1546,27 +1553,38 @@ __device__ bool hullHullGroup(EngineState &S, const PairSetup &ps, HullScratch &
         do {
             const HalfEdge cur = inc_mesh.halfEdges[he];
             he = cur.next;
-            if (n < kClipCap) src[n++] = inc_verts[cur.rootVertex];
+            if (n == kMaxFaceVerts) {
+                n = -1;
+                break;
+            }
+            src[n++] = inc_verts[cur.rootVertex];
         } while (he != start);
         he = ref_mesh.faceBaseHalfEdges[ref_face];
         start = he;
         Vector3 cur_pt = ref_verts[ref_mesh.halfEdges[he].rootVertex];
-        do {
+        int sides = 0;
+        while (n >= 0) {
+            if (++sides > kMaxFaceVerts) {
+                n = -1;
+                break;
+            }
             he = ref_mesh.halfEdges[he].next;
             Vector3 next_pt = ref_verts[ref_mesh.halfEdges[he].rootVertex];
             Vector3 side_n = cross(next_pt - cur_pt, ref_plane.normal);
             Plane side { side_n, dot(side_n, cur_pt) };
             cur_pt = next_pt;
-            n = n > 0 ? clipAgainst(dst, side, src, n) : 0;
-            if (n > kClipCap) n = kClipCap;
+            if (n > 0) n = clipAgainst(dst, side, src, n, kClipCap);
             Vector3 *tmp = src;
             src = dst;
             dst = tmp;
             in_b ^= 1;
-        } while (he != start);
+            if (he == start) break;
+        }
+        if (n < 0) atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
     }
     const int leader = __ffs(gm) - 1;
     n = __shfl_sync(gm, n, leader);
+    if (n < 0) return false;
     in_b = __shfl_sync(gm, in_b, leader);
     __syncwarp(gm);
     const int count = groupManifold<kGroupLanes>(gm, sub, ref_plane, in_b ? scratch.clipB : scratch.clipA, n,

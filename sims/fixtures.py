@@ -106,6 +106,31 @@ def _triggers_objects():
     return triggers_objects()
 
 
+def _hullpile_objects():
+    from .objects import hullpile_objects
+    return hullpile_objects()
+
+
+def _hullpile_desc(name, bodies, compile_flags=()):
+    return SimDesc(
+        name=name,
+        sources=[os.path.join(_ROOT, "hullpile", "sim.cpp")],
+        num_exports=6,
+        num_taskgraphs=1,
+        inputs=[],
+        outputs=[Slot(0, "body_pos", "float32", (bodies, 3)), Slot(1, "body_rot", "float32", (bodies, 4)),
+                 Slot(2, "body_vel", "float32", (bodies, 6)), Slot(3, "body_entity", "int32", (bodies, 2)),
+                 Slot(4, "body_scale", "float32", (bodies, 3)), Slot(5, "body_object", "int32", (bodies,))],
+        # layout: 0 the pile, 1 / 2 one prism resting face down on a pedestal / the plane
+        pack_config=lambda cfg: struct.pack("<QII", int(cfg.get("obj_mgr_ptr", 0)), int(cfg["layout"]), 0),
+        pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
+        oracle_extra=lambda cfg: [int(cfg.get("seed", 0))],
+        defaults={"seed": 0, "layout": 0},
+        objects=_hullpile_objects,
+        compile_flags=list(compile_flags),
+    )
+
+
 def _image_size(cfg, default_res):
     """Render config image size from the fixture config: keyword arguments for the
     render_assets builders.  `width` and `height` (both) give non-square images, else the
@@ -283,6 +308,11 @@ SIMS: Dict[str, SimDesc] = {
         objects=_balls_objects,
         compile_flags=["-DBALLS_MANY=1"],
     ),
+    # hulls at the narrowphase's staging caps (16 vertices, 16 faces, 8-vertex faces), compound
+    # bodies in the solver, physics only (tests/test_hullpile.py)
+    "hullpile": _hullpile_desc("hullpile", 20),
+    # build variant with 60 bodies per world (hull contacts past the 48 staged bodies)
+    "hullpile_many": _hullpile_desc("hullpile_many", 60, ["-DHULLPILE_MANY=1"]),
     # GPU only: batch ray caster with a real TLAS / BLAS, materials, lights (tests/test_render_bvh.py)
     "gallery": SimDesc(
         name="gallery",

@@ -214,6 +214,33 @@ def hex_prism_half_edge_mesh():
     return build_half_edge_mesh(v, orient_faces(v, faces))
 
 
+def bipyramid_half_edge_mesh(n: int = 8):
+    """n-gon bipyramid: ring of circumradius 0.5 at z = 0, apexes at z = +-0.6 (n + 2
+    vertices, 2n triangles, 3n edges; n = 8 is at the engine's 16-face hull cap)."""
+    ang = 2.0 * np.pi * np.arange(n) / n
+    v = np.array([[0.5 * np.cos(a), 0.5 * np.sin(a), 0.0] for a in ang] + [[0, 0, 0.6], [0, 0, -0.6]],
+                 dtype=np.float32)
+    faces = [[i, (i + 1) % n, n] for i in range(n)] + [[i, (i + 1) % n, n + 1] for i in range(n)]
+    return build_half_edge_mesh(v, orient_faces(v, faces))
+
+
+def pyramid_half_edge_mesh(n: int, apex=(0.0, 0.0)):
+    """n-gon pyramid: base of circumradius 0.5 at z = -0.5, apex at (apex, 0.5) (n + 1
+    vertices, n + 1 faces).  An off-centre apex leaves no two faces parallel."""
+    ang = 2.0 * np.pi * np.arange(n) / n
+    v = np.array([[0.5 * np.cos(a), 0.5 * np.sin(a), -0.5] for a in ang] + [[apex[0], apex[1], 0.5]],
+                 dtype=np.float32)
+    faces = [list(range(n))] + [[i, (i + 1) % n, n] for i in range(n)]
+    return build_half_edge_mesh(v, orient_faces(v, faces))
+
+
+def tetra_half_edge_mesh():
+    """An irregular tetrahedron, vertices relative to their mean."""
+    v = np.array([[0.55, -0.2, -0.3], [-0.4, 0.5, -0.3], [-0.3, -0.45, -0.25], [0.05, 0.1, 0.55]])
+    v = (v - v.mean(axis=0)).astype(np.float32)
+    return build_half_edge_mesh(v, orient_faces(v, [[0, 1, 2], [0, 1, 3], [1, 2, 3], [0, 2, 3]]))
+
+
 def build_objects(specs, plane_extent: float = 1.0e5) -> Tuple[bytes, List[int]]:
     """specs: one dict per object -- {"mesh": <half-edge mesh dict> | "plane" | ("sphere", r),
     "meta": bytes(52)}; one primitive per object.  Same blob layout as room_objects()."""
@@ -379,6 +406,47 @@ def shifted_box_half_edge_mesh(dx: float, dy: float, dz: float):
     v = box["vertices"] + np.array([dx, dy, dz], dtype=np.float32)
     faces = [[0, 2, 3, 1], [4, 5, 7, 6], [0, 1, 5, 4], [2, 6, 7, 3], [0, 4, 6, 2], [1, 3, 7, 5]]
     return build_half_edge_mesh(v, faces)
+
+
+def hullpile_objects(big_face: bool = False) -> Tuple[bytes, List[int]]:
+    return build_compound_objects(hullpile_specs(big_face))
+
+
+def hullpile_specs(big_face: bool = False):
+    """Objects of sims/hullpile, in SimObject order: Box, Wedge, OctPrism (16 vertices, two
+    8-vertex faces), Bipyramid (16 faces), Tetra, PentaPyramid (off-centre apex), Ball
+    (radius 0.5), Dumbbell (two boxes 1.2 apart), CappedBox (a box below the origin and a
+    sphere of radius 0.45 at it: a sphere primitive has no offset), Plane, Wall (static box),
+    Pedestal (static octagonal prism).  Inertia tensors are those of the bounding box at unit
+    scale.  big_face: OctPrism and Pedestal are 11-gon pyramids instead (12 vertices and 12
+    faces, inside the hull caps, but an 11-vertex base: tests/test_cliffs.py)."""
+    box, wedge = box_half_edge_mesh(), wedge_half_edge_mesh()
+    prism = pyramid_half_edge_mesh(11) if big_face else ngon_prism_half_edge_mesh(8)
+    static = _metadata(0.0, [0.0, 0.0, 0.0], 0.5, 0.5)
+
+    def dyn(mass, sx, sy, sz):
+        return _metadata(np.float32(1.0 / mass), _box_inv_inertia(mass, sx, sy, sz), 0.5, 0.5)
+
+    ball_m, ball_r = 3.0, 0.5
+    ball_inv_i = np.float32(1.0 / (0.4 * ball_m * ball_r * ball_r))
+    specs = [
+        dict(prims=[box], meta=dyn(4.0, 1.0, 1.0, 1.0)),                                     # Box
+        dict(prims=[wedge], meta=dyn(4.0, 1.0, 1.0, 1.0)),                                   # Wedge
+        dict(prims=[prism], meta=dyn(6.0, 1.0, 1.0, 1.0)),                                   # OctPrism
+        dict(prims=[bipyramid_half_edge_mesh(8)], meta=dyn(4.0, 1.0, 1.0, 1.2)),            # Bipyramid
+        dict(prims=[tetra_half_edge_mesh()], meta=dyn(2.0, 0.95, 0.95, 0.85)),               # Tetra
+        dict(prims=[pyramid_half_edge_mesh(5, (0.15, 0.1))], meta=dyn(3.0, 1.0, 1.0, 1.0)),  # PentaPyramid
+        dict(prims=[("sphere", ball_r)], meta=_metadata(np.float32(1.0 / ball_m),           # Ball
+                                                        [ball_inv_i] * 3, 0.5, 0.5)),
+        dict(prims=[shifted_box_half_edge_mesh(-0.6, 0.0, 0.0),                              # Dumbbell
+                    shifted_box_half_edge_mesh(0.6, 0.0, 0.0)], meta=dyn(6.0, 2.2, 1.0, 1.0)),
+        dict(prims=[shifted_box_half_edge_mesh(0.0, 0.0, -0.5), ("sphere", 0.45)],          # CappedBox
+             meta=dyn(5.0, 1.0, 1.0, 1.45)),
+        dict(prims=["plane"], meta=static),                                                  # Plane
+        dict(prims=[box], meta=static),                                                      # Wall
+        dict(prims=[prism], meta=static),                                                    # Pedestal
+    ]
+    return specs
 
 
 def triggers_objects() -> Tuple[bytes, List[int]]:

@@ -41,6 +41,10 @@ CASES = [
     ("balls_w6_s160", "balls", 6, 160, {"seed": 3}),
     # 95 bodies per world: candidate search beyond one 64-leaf mask word, ~300 contacts per world
     ("balls_many_w2_s60", "balls_many", 2, 60, {"seed": 9}),
+    # hulls at the narrowphase's staging caps, compound bodies, spheres inside hulls
+    ("hullpile_w4_s150", "hullpile", 4, 150, {"seed": 41}),
+    # 60 bodies per world: hull contacts on bodies the position solve does not stage
+    ("hullpile_many_w2_s100", "hullpile_many", 2, 100, {"seed": 43}),
 ]
 
 if __name__ == "__main__":
@@ -54,11 +58,16 @@ if __name__ == "__main__":
         print(name, {k: (v.shape if not isinstance(v, list) else f"{len(v)} frames")
                      for k, v in outs.items()})
 
-    # per-column digests of the reference traces of trace_utils.REFERENCE_CASES
-    if not only or "reference_digests" in only:
+    # per-column digests of the reference traces of trace_utils.REFERENCE_CASES (all of
+    # them; or, named on the command line, only those, merged into the existing file)
+    named = [name for name in only if name in REFERENCE_CASES]
+    if not only or "reference_digests" in only or named:
         import json
         digests = {}
-        for name in REFERENCE_CASES:
+        if named and "reference_digests" not in only:
+            with open(DIGESTS_PATH) as f:
+                digests = json.load(f)
+        for name in (named or REFERENCE_CASES):
             sim, W, steps, inputs, cfg = reference_case(name)
             outs, _ = run_reference(SIMS[sim], W, steps, inputs, cfg, workers=4)
             digests[name] = trace_digests(reference_columns(name, outs))

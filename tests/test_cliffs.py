@@ -101,6 +101,43 @@ def test_hull_vertex_cap():
     ex.close()
 
 
+@pytest.mark.gpu
+@pytest.mark.parametrize("layout", [1, 2], ids=["hull_on_hull", "hull_on_plane"])
+def test_hull_face_vertex_cap(layout):
+    # 11-gon pyramids: 12 vertices and 12 faces, inside the hull caps, but an 11-vertex
+    # base.  Base to base on an upside-down static one at a relative yaw of pi / 11 (a
+    # hull - hull pair whose clip would make 22 points: tests/test_hull_clip_model.py), or
+    # base down on the plane (the incident face of a hull - plane pair): both must raise
+    # at step 0, not overrun the 8-vertex face staging or the 20-point clip buffers
+    from functools import partial
+    from sims import make_executor
+    from sims.objects import hullpile_objects
+    ex = make_executor("hullpile", 8, objects_fn=partial(hullpile_objects, big_face=True), layout=layout, seed=1)
+    graph = ex.buildLaunchGraphAllTaskGraphs()
+    step, msg = _run_until_error(ex, graph, 2)
+    assert step == 0 and "physics buffer overflow" in msg, (step, msg)
+    _device_still_healthy()
+    ex.close()
+
+
+@pytest.mark.gpu
+def test_hull_face_on_face_at_the_cap_runs():
+    # the same two layouts with the octagonal prism: 8-vertex faces are within the cap
+    from sims import make_executor
+    for layout in (1, 2):
+        ex = make_executor("hullpile", 8, layout=layout, seed=1)
+        graph = ex.buildLaunchGraphAllTaskGraphs()
+        step, msg = _run_until_error(ex, graph, 10)
+        assert step is None, (layout, step, msg)
+        rows = ex.exportedNumRows(0)
+        assert rows == 8 * (3 if layout == 1 else 2)
+        pos = ex.tensor(0, "float32", (rows, 3)).cpu().numpy().reshape(8, -1, 3)
+        # the prism (each world's last body) rests on the pedestal's face (z = 1.5) or on
+        # the plane, its centre 0.5 above
+        assert np.allclose(pos[:, -1, 2], 2.0 if layout == 1 else 0.5, atol=0.05), pos[:, -1]
+        ex.close()
+
+
 # ---- table growth (role of the reference's VM-backed tables, src/mw/device/state.cpp:29-80) ----
 
 @pytest.mark.gpu

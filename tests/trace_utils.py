@@ -48,7 +48,7 @@ def make_inputs(sim: str, num_worlds: int, num_steps: int, seed: int = 0) -> Dic
             "reset": (rng.random((num_steps, num_worlds, 1)) < 0.004).astype(np.int32),
             "action": act.astype(np.int32),
         }
-    if sim in ("balls", "balls_many"):
+    if sim in ("balls", "balls_many", "hullpile", "hullpile_many"):
         return {}          # physics only: no inputs
     raise KeyError(sim)
 
@@ -153,9 +153,12 @@ REFERENCE_CASES = {
     "arena_w48_s70": ("arena", 48, 70, 77, {"episode_len": 45, "seed": 11}),
     "balls_w400_s150": ("balls", 400, 150, None, {"seed": 7000}),
     "balls_many_w48_s80": ("balls_many", 48, 80, None, {"seed": 31000}),
+    "hullpile_w300_s120": ("hullpile", 300, 120, None, {"seed": 52000}),
+    "hullpile_many_w48_s100": ("hullpile_many", 48, 100, None, {"seed": 53000}),
+    "hullpile_w64_s60": ("hullpile", 64, 60, None, {"seed": 54000}),
 }
-# checked on the first worlds of a larger GPU run (tests/test_full_size.py)
-PREFIX_CASES = {"gridworld_w128_s60", "room_w64_s60", "arena_w48_s70"}
+# checked on the first worlds of a larger GPU run (tests/test_full_size.py, tests/test_hullpile.py)
+PREFIX_CASES = {"gridworld_w128_s60", "room_w64_s60", "arena_w48_s70", "hullpile_w64_s60"}
 DIGESTS_PATH = os.path.join(GOLDEN_DIR, "reference_digests.json")
 
 
@@ -181,11 +184,12 @@ def trace_digests(outs) -> Dict[str, str]:
 
 def reference_columns(name, outs):
     """The columns of a reference trace that the GPU test of `name` compares: the cases of
-    PREFIX_CASES roll out only the fixed-size columns."""
+    PREFIX_CASES roll out only the fixed-size columns, and no entity handles (they come
+    from one pool for all worlds, so they depend on the number of worlds)."""
     if name not in PREFIX_CASES:
         return dict(outs)
     dynamic = {s.name for s in SIMS[REFERENCE_CASES[name][0]].outputs if s.dynamic}
-    return {k: v for k, v in outs.items() if k not in dynamic}
+    return {k: v for k, v in outs.items() if k not in dynamic and not k.endswith("entity")}
 
 
 def assert_matches_reference(name, got, exact=True, rtol=1e-4, atol=1e-5):
