@@ -14,13 +14,14 @@
 //   renderLightKernels           carriers refresh their LightDesc, lights gathered per world
 //   renderGatherViewsKernel      PerspectiveCameraData per view
 //   renderBuildTLASKernel        worlds of <= kWarpTLASInstances: ONE WARP PER WORLD, all in
-//                                shared memory: 30-bit Morton codes of the box centres inside
-//                                the world's bounds, rank sort, Karras' parallel LBVH,
-//                                bottom-up boxes, collapse to 4-wide nodes, quantise ->
-//                                QBVHNode[] (the reference's traversal format)
-//   renderBuildLargeTLASKernel   larger worlds: the same tree, one block per world taken by
-//                                ticket, scratch in global memory, bitonic key sort staged
-//                                through shared memory in kSortChunk tiles
+//                                shared memory, rank sort
+//   renderBuildLargeTLASKernel   larger worlds: one block per world taken by ticket, scratch
+//                                in global memory, bitonic key sort staged through shared
+//                                memory in kSortChunk tiles
+//   Both build the same tree by calling the same rule functions (centreBounds, mortonKey,
+//   karrasSplit, mergeBoxes, expandWide, writeWideNode): 30-bit Morton codes of the box
+//   centres inside the world's bounds, Karras' parallel LBVH, bottom-up boxes, collapse to
+//   4-wide nodes, quantise -> QBVHNode[] (the reference's traversal format)
 // Render graph: renderRaycastKernel, one thread per pixel, one block per view
 // (8 x 4 pixel tiles per warp): TLAS -> instance -> object-space ray -> BLAS
 // (reference-format MeshBVH: quantised 4-wide nodes over de-indexed triangles)
@@ -64,7 +65,6 @@ struct RenderHost {
     RenderState *dRender = nullptr;
     RenderState hRender;
     bool active = false;
-    size_t tlasSmem = 0;
     // instance list, TLAS nodes, large-world key / node scratch: one entry per renderable row
     VMRange instanceRange, nodeRange, keyRange, buildRange;
 };
@@ -84,6 +84,12 @@ struct TLASBuildNode {
 constexpr int kWarpTLASInstances = 128;
 constexpr int kLargeTLASThreads = 512;
 constexpr int kSortChunk = 4096;        // keys sorted per shared-memory pass (32 KiB)
+
+// a world of n instances builds its TLAS in renderBuildLargeTLASKernel, else in renderBuildTLASKernel
+__device__ __forceinline__ bool largeTLASWorld(i32 n)
+{
+    return n > kWarpTLASInstances;
+}
 
 // Visible renderable of world w at `row`: the row belongs to w and its Renderable names an entity
 __device__ __forceinline__ bool renderableVisible(const TableDesc &t, const RenderArchetype &ra, i32 row, i32 w)
@@ -148,7 +154,7 @@ renderScanInstancesKernel(EngineState *Sp)
         for (int k = 0; k < kScanWorlds; k++) {
             counts[k] = first + k < W ? R.instanceCounts[first + k] : 0;
             n += counts[k];
-            large += counts[k] > kWarpTLASInstances ? 1 : 0;
+            large += largeTLASWorld(counts[k]) ? 1 : 0;
         }
         i32 a = n, b = large;
         for (int o = 1; o < 32; o <<= 1) {
@@ -183,7 +189,7 @@ renderScanInstancesKernel(EngineState *Sp)
             const i32 w = first + k;
             if (w < W) {
                 R.instanceOffsets[w] = (i32)min(off, (long long)R.instanceCapacity);
-                if (counts[k] > kWarpTLASInstances) R.largeWorlds[slot++] = w;
+                if (largeTLASWorld(counts[k])) R.largeWorlds[slot++] = w;
             }
             off += counts[k];
         }
@@ -379,23 +385,19 @@ __device__ __forceinline__ RayShear rayShear(Vector3 d, Diag3x3 inv_d)
 }
 
 // ---- render-prepare: per-world TLAS ----------------------------------------------------------
-// One warp per world; everything lives in the warp's slice of dynamic shared
-// memory until the 4-wide nodes are written out.
-struct TLASScratch {
-    unsigned long long *keys;     // [n] morton << 32 | gather index
-    float *leafBox;               // [n][6] in SORTED order
-    float *nodeBox;               // [n - 1][6] binary internal nodes
-    short *left, *right;          // [n - 1] child: >= 0 internal, < 0: ~leaf (sorted position)
-    short *parent;                // [2n - 1]: internal nodes first, then leaves
-    int *flags;                   // [n - 1] arrival counters of the bottom-up pass
-    short *wideBin;               // [n] binary node of each wide node
-    int *order;                   // [n] sorted position -> gather index
-};
-
-__host__ __device__ inline size_t tlasScratchBytes(int n)
-{
-    return (size_t)n * (8 + 24 + 24 + 2 + 2 + 4 + 4 + 2 + 4) + 64;
-}
+// Two builders make the same tree; largeTLASWorld() says which one owns a world.  They differ
+// in the key sort, where the scratch lives and the fences that go with it.  The build rules are
+// the functions below, which both call (binary children: >= 0 internal node, < 0 ~leaf, the
+// leaf's sorted position):
+//   centreBounds   bounds of the instance box centres (per thread, then across the warp)
+//   mortonKey      10-bit-per-axis Morton code of a box centre << 32 | gather index
+//   karrasSplit    Karras 2012: the two children of internal node i over the sorted keys
+//   mergeBoxes     bottom-up box of a binary node: fminf / fmaxf of its children's
+//   expandWide     4-wide collapse: expand the inner child of largest wideChildArea, first
+//                  maximum wins
+//   writeWideNode  one QBVHNode: quantizeNode, leaves as 0x80000000 | gather index, inner
+//                  children numbered by the caller
+// tests/tlas_model.py restates the same rules in numpy.
 
 __device__ __forceinline__ u32 expandBits10(u32 v)
 {
@@ -412,12 +414,141 @@ __device__ __forceinline__ int commonPrefix(const unsigned long long *keys, int 
     return __clzll((long long)(keys[i] ^ keys[j]));     // keys are unique (index in the low word)
 }
 
-// Surface-area measure the 4-wide collapse ranks inner children by: dx*dy + dy*dz + dz*dx
-// with its fmas spelled out, so both builders (and tests/tlas_model.py) round it alike.
-__device__ __forceinline__ float wideChildArea(const float *b)
+// Bounds of the box centres of instances first, first + stride, ... < n, reduced across the warp
+__device__ __forceinline__ void centreBounds(const RenderInstance *inst, int n, int first, int stride,
+                                             float lo[3], float hi[3])
 {
-    const float dx = b[3] - b[0], dy = b[4] - b[1], dz = b[5] - b[2];
+    for (int a = 0; a < 3; a++) {
+        lo[a] = FLT_MAX;
+        hi[a] = -FLT_MAX;
+    }
+    for (int i = first; i < n; i += stride) {
+        for (int a = 0; a < 3; a++) {
+            const float c = 0.5f * (inst[i].aabbMin[a] + inst[i].aabbMax[a]);
+            lo[a] = fminf(lo[a], c);
+            hi[a] = fmaxf(hi[a], c);
+        }
+    }
+    for (int o = 16; o >= 1; o >>= 1) {
+        for (int a = 0; a < 3; a++) {
+            lo[a] = fminf(lo[a], __shfl_xor_sync(0xffffffffu, lo[a], o));
+            hi[a] = fmaxf(hi[a], __shfl_xor_sync(0xffffffffu, hi[a], o));
+        }
+    }
+}
+
+// Key of instance i (its gather index): Morton code of its box centre inside the world's centre
+// bounds << 32 | i, so keys are unique and any correct sort gives one order
+__device__ __forceinline__ unsigned long long mortonKey(const RenderInstance &ri, u32 i, const float lo[3],
+                                                        const float hi[3])
+{
+    u32 code = 0;
+    for (int a = 0; a < 3; a++) {
+        const float c = 0.5f * (ri.aabbMin[a] + ri.aabbMax[a]);
+        const float ext = hi[a] - lo[a];
+        float u = ext > 0.f ? (c - lo[a]) / ext : 0.f;
+        u = fminf(fmaxf(u * 1024.f, 0.f), 1023.f);
+        code |= expandBits10((u32)u) << a;
+    }
+    return ((unsigned long long)code << 32) | i;
+}
+
+// Karras 2012: internal node i of the n - 1 covers a range of the n sorted keys -> its children
+__device__ __forceinline__ int2 karrasSplit(const unsigned long long *keys, int n, int i)
+{
+    const int d = commonPrefix(keys, n, i, i + 1) - commonPrefix(keys, n, i, i - 1) >= 0 ? 1 : -1;
+    const int delta_min = commonPrefix(keys, n, i, i - d);
+    int lmax = 2;
+    while (commonPrefix(keys, n, i, i + lmax * d) > delta_min) lmax <<= 1;
+    int l = 0;
+    for (int t = lmax >> 1; t >= 1; t >>= 1) {
+        if (commonPrefix(keys, n, i, i + (l + t) * d) > delta_min) l += t;
+    }
+    const int j = i + l * d;
+    const int delta_node = commonPrefix(keys, n, i, j);
+    int s = 0;
+    for (int t = (l + 1) >> 1; ; t = (t + 1) >> 1) {
+        if (commonPrefix(keys, n, i, i + (s + t) * d) > delta_node) s += t;
+        if (t == 1) break;
+    }
+    const int gamma = i + s * d + min(d, 0);
+    const int first = min(i, j), last = max(i, j);
+    return make_int2(first == gamma ? ~gamma : gamma, last == gamma + 1 ? ~(gamma + 1) : gamma + 1);
+}
+
+// In the helpers below box(c, a) is float a (min xyz, max xyz) of binary child c's box and
+// children(b) the two children of internal node b.
+
+// Box of a binary node with children lc, rc
+template <class Box>
+__device__ __forceinline__ void mergeBoxes(float *dst, int lc, int rc, Box box)
+{
+    float b[6];
+    for (int a = 0; a < 6; a++) {
+        const float lv = box(lc, a), rv = box(rc, a);
+        b[a] = a < 3 ? fminf(lv, rv) : fmaxf(lv, rv);
+    }
+    for (int a = 0; a < 6; a++) dst[a] = b[a];
+}
+
+// Surface-area measure the 4-wide collapse ranks inner child c by: dx*dy + dy*dz + dz*dx with
+// its fmas spelled out, so FMA contraction (this file is compiled with it) cannot change how it
+// rounds and tests/tlas_model.py can restate it exactly.
+template <class Box>
+__device__ __forceinline__ float wideChildArea(int c, Box box)
+{
+    const float dx = box(c, 3) - box(c, 0), dy = box(c, 4) - box(c, 1), dz = box(c, 5) - box(c, 2);
     return __fmaf_rn(dx, dz, __fmaf_rn(dx, dy, __fmul_rn(dy, dz)));
+}
+
+// Children of the wide node over internal node bin: its two, then the inner child of largest
+// area replaced by its own two until there are kBVHWidth or only leaves -> their count
+template <class Children, class Box>
+__device__ __forceinline__ int expandWide(int kids[kBVHWidth], int bin, Children children, Box box)
+{
+    const int2 two = children(bin);
+    kids[0] = two.x;
+    kids[1] = two.y;
+    int nk = 2;
+    while (nk < kBVHWidth) {
+        int pick = -1;
+        float best = -1.f;
+        for (int c = 0; c < nk; c++) {
+            if (kids[c] < 0) continue;
+            const float area = wideChildArea(kids[c], box);
+            if (area > best) {
+                best = area;
+                pick = c;
+            }
+        }
+        if (pick < 0) break;
+        const int2 split = children(kids[pick]);
+        kids[pick] = split.x;
+        kids[nk++] = split.y;
+    }
+    return nk;
+}
+
+// Writes the wide node with children kids[0, nk): a leaf is 0x80000000 | gatherIndex(sorted
+// position), an inner child the wide-node id newNode(binary node) hands out, in child order
+template <class Box, class GatherIndex, class NewNode>
+__device__ __forceinline__ void writeWideNode(QBVHNode *dst, const int *kids, int nk, Box box,
+                                              GatherIndex gatherIndex, NewNode newNode)
+{
+    float cmin[kBVHWidth][3], cmax[kBVHWidth][3];
+    for (int c = 0; c < nk; c++) {
+        for (int a = 0; a < 3; a++) {
+            cmin[c][a] = box(kids[c], a);
+            cmax[c][a] = box(kids[c], 3 + a);
+        }
+    }
+    QBVHNode node;
+    quantizeNode(node, nk, cmin, cmax);
+    for (int c = 0; c < nk; c++) {
+        node.triSize[c] = 0;
+        node.childrenIdx[c] = kids[c] < 0 ? 0x80000000u | gatherIndex(~kids[c]) : (u32)newNode(kids[c]);
+    }
+    *dst = node;
 }
 
 // Traversal budget (traceWorld): kTraceStack entries per ray, shared by the TLAS and the
@@ -435,16 +566,31 @@ __device__ __forceinline__ void recordTLASDepth(EngineState &S, RenderState &R, 
     if (depth > kMaxTLASDepth && n > kFlatInstances) atomicOr(&S.errorFlags, (u32)ErrRenderTLASDepth);
 }
 
+// renderBuildTLASKernel's scratch: the warp's slice of dynamic shared memory, sized for the
+// largest world the warp builder owns
+struct TLASScratch {
+    unsigned long long keys[kWarpTLASInstances];    // morton << 32 | gather index, sorted in place
+    float leafBox[kWarpTLASInstances * 6];          // in SORTED order
+    float nodeBox[kWarpTLASInstances * 6];          // binary internal nodes
+    int flags[kWarpTLASInstances];                  // arrival counters of the bottom-up pass
+    int order[kWarpTLASInstances];                  // sorted position -> gather index
+    short left[kWarpTLASInstances], right[kWarpTLASInstances];  // children of the internal nodes
+    short parent[2 * kWarpTLASInstances];           // internal nodes first, then leaves
+    short wideBin[kWarpTLASInstances];              // binary node of each wide node
+};
+constexpr size_t kTLASScratchBytes = sizeof(TLASScratch) + 64;     // 64 B of slack past the layout
+
 __global__ void __launch_bounds__(32)
 renderBuildTLASKernel(EngineState *Sp)
 {
     extern __shared__ __align__(16) unsigned char tlas_smem[];
+    TLASScratch &sc = *reinterpret_cast<TLASScratch *>(tlas_smem);
     EngineState &S = *Sp;
     RenderState &R = *S.render;
     const int lane = threadIdx.x;
     const i32 w = (i32)blockIdx.x;
     const i32 n = R.instanceCounts[w];
-    if (n > kWarpTLASInstances) return;         // renderBuildLargeTLASKernel's
+    if (largeTLASWorld(n)) return;
     const i32 offset = R.instanceOffsets[w];
     const RenderInstance *inst = R.instances + offset;
     QBVHNode *out = R.tlasNodes + offset;
@@ -455,47 +601,11 @@ renderBuildTLASKernel(EngineState *Sp)
         }
         return;
     }
-    const int cap = kWarpTLASInstances;
-    TLASScratch sc;
-    {
-        unsigned char *p = tlas_smem;
-        sc.keys = (unsigned long long *)p; p += (size_t)cap * 8;
-        sc.leafBox = (float *)p; p += (size_t)cap * 24;
-        sc.nodeBox = (float *)p; p += (size_t)cap * 24;
-        sc.flags = (int *)p; p += (size_t)cap * 4;
-        sc.order = (int *)p; p += (size_t)cap * 4;
-        sc.left = (short *)p; p += (size_t)cap * 2;
-        sc.right = (short *)p; p += (size_t)cap * 2;
-        sc.parent = (short *)p; p += (size_t)cap * 4;
-        sc.wideBin = (short *)p;
-    }
 
     // 1. world bounds of the box centres, Morton keys
-    float lo[3] = { FLT_MAX, FLT_MAX, FLT_MAX }, hi[3] = { -FLT_MAX, -FLT_MAX, -FLT_MAX };
-    for (int i = lane; i < n; i += 32) {
-        for (int a = 0; a < 3; a++) {
-            const float c = 0.5f * (inst[i].aabbMin[a] + inst[i].aabbMax[a]);
-            lo[a] = fminf(lo[a], c);
-            hi[a] = fmaxf(hi[a], c);
-        }
-    }
-    for (int o = 16; o >= 1; o >>= 1) {
-        for (int a = 0; a < 3; a++) {
-            lo[a] = fminf(lo[a], __shfl_xor_sync(0xffffffffu, lo[a], o));
-            hi[a] = fmaxf(hi[a], __shfl_xor_sync(0xffffffffu, hi[a], o));
-        }
-    }
-    for (int i = lane; i < n; i += 32) {
-        u32 code = 0;
-        for (int a = 0; a < 3; a++) {
-            const float c = 0.5f * (inst[i].aabbMin[a] + inst[i].aabbMax[a]);
-            const float ext = hi[a] - lo[a];
-            float u = ext > 0.f ? (c - lo[a]) / ext : 0.f;
-            u = fminf(fmaxf(u * 1024.f, 0.f), 1023.f);
-            code |= expandBits10((u32)u) << a;
-        }
-        sc.keys[i] = ((unsigned long long)code << 32) | (u32)i;
-    }
+    float lo[3], hi[3];
+    centreBounds(inst, n, lane, 32, lo, hi);
+    for (int i = lane; i < n; i += 32) sc.keys[i] = mortonKey(inst[i], (u32)i, lo, hi);
     __syncwarp();
 
     // 2. rank sort (n is tens to a few hundred): sorted position of every instance
@@ -529,49 +639,27 @@ renderBuildTLASKernel(EngineState *Sp)
     }
     __syncwarp();
 
+    auto box = [&](int c, int a) { return c >= 0 ? sc.nodeBox[c * 6 + a] : sc.leafBox[(~c) * 6 + a]; };
+    auto gatherIndex = [&](int pos) { return (u32)sc.order[pos]; };
+    // a world of one instance has no internal node: its root holds the leaf alone (and no
+    // inner child to number)
     if (n == 1) {
         if (lane == 0) {
-            float cmin[kBVHWidth][3], cmax[kBVHWidth][3];
-            for (int a = 0; a < 3; a++) {
-                cmin[0][a] = sc.leafBox[a];
-                cmax[0][a] = sc.leafBox[3 + a];
-            }
-            QBVHNode node;
-            quantizeNode(node, 1, cmin, cmax);
-            node.childrenIdx[0] = 0x80000000u | (u32)sc.order[0];
-            node.triSize[0] = 0;
-            out[0] = node;
+            const int leaf = ~0;
+            writeWideNode(out, &leaf, 1, box, gatherIndex, [](int) { return 0; });
             R.tlasNodeCounts[w] = 1;
             recordTLASDepth(S, R, w, n, 1);
         }
         return;
     }
 
-    // 3. Karras 2012: internal node i covers a key range; leaves are sorted positions
+    // 3. internal nodes and parents
     for (int i = lane; i < n - 1; i += 32) {
-        const int d = commonPrefix(sc.keys, n, i, i + 1) - commonPrefix(sc.keys, n, i, i - 1) >= 0 ? 1 : -1;
-        const int delta_min = commonPrefix(sc.keys, n, i, i - d);
-        int lmax = 2;
-        while (commonPrefix(sc.keys, n, i, i + lmax * d) > delta_min) lmax <<= 1;
-        int l = 0;
-        for (int t = lmax >> 1; t >= 1; t >>= 1) {
-            if (commonPrefix(sc.keys, n, i, i + (l + t) * d) > delta_min) l += t;
-        }
-        const int j = i + l * d;
-        const int delta_node = commonPrefix(sc.keys, n, i, j);
-        int s = 0;
-        for (int t = (l + 1) >> 1; ; t = (t + 1) >> 1) {
-            if (commonPrefix(sc.keys, n, i, i + (s + t) * d) > delta_node) s += t;
-            if (t == 1) break;
-        }
-        const int gamma = i + s * d + min(d, 0);
-        const int first = min(i, j), last = max(i, j);
-        const int lc = first == gamma ? ~gamma : gamma;             // leaf: ~position
-        const int rc = last == gamma + 1 ? ~(gamma + 1) : gamma + 1;
-        sc.left[i] = (short)lc;
-        sc.right[i] = (short)rc;
-        sc.parent[lc >= 0 ? lc : (n - 1) + (~lc)] = (short)i;
-        sc.parent[rc >= 0 ? rc : (n - 1) + (~rc)] = (short)i;
+        const int2 c = karrasSplit(sc.keys, n, i);
+        sc.left[i] = (short)c.x;
+        sc.right[i] = (short)c.y;
+        sc.parent[c.x >= 0 ? c.x : (n - 1) + (~c.x)] = (short)i;
+        sc.parent[c.y >= 0 ? c.y : (n - 1) + (~c.y)] = (short)i;
         sc.flags[i] = 0;
     }
     if (lane == 0) sc.parent[0] = -1;
@@ -583,13 +671,7 @@ renderBuildTLASKernel(EngineState *Sp)
         while (node >= 0) {
             __threadfence_block();
             if (atomicAdd(&sc.flags[node], 1) == 0) break;
-            const int lc = sc.left[node], rc = sc.right[node];
-            const float *lb = lc >= 0 ? sc.nodeBox + lc * 6 : sc.leafBox + (~lc) * 6;
-            const float *rb = rc >= 0 ? sc.nodeBox + rc * 6 : sc.leafBox + (~rc) * 6;
-            for (int a = 0; a < 3; a++) {
-                sc.nodeBox[node * 6 + a] = fminf(lb[a], rb[a]);
-                sc.nodeBox[node * 6 + 3 + a] = fmaxf(lb[3 + a], rb[3 + a]);
-            }
+            mergeBoxes(sc.nodeBox + node * 6, sc.left[node], sc.right[node], box);
             node = sc.parent[node];
         }
     }
@@ -603,6 +685,7 @@ renderBuildTLASKernel(EngineState *Sp)
     }
     __syncwarp();
     int depth = 1;
+    auto children = [&](int b) { return make_int2(sc.left[b], sc.right[b]); };
     // waves: nodes [done, count) exist and are not written yet; writing them appends
     // their inner children behind `count`
     for (int done = 0;;) {
@@ -611,51 +694,16 @@ renderBuildTLASKernel(EngineState *Sp)
         const int k = done + lane;
         __syncwarp();
         if (k < count_now) {
-            const int bin = sc.wideBin[k];
             const int level = k == 0 ? 1 : sc.flags[k];
             int kids[kBVHWidth];
-            int nk = 2;
-            kids[0] = sc.left[bin];
-            kids[1] = sc.right[bin];
-            while (nk < kBVHWidth) {
-                int pick = -1;
-                float best = -1.f;
-                for (int c = 0; c < nk; c++) {
-                    if (kids[c] < 0) continue;
-                    const float area = wideChildArea(sc.nodeBox + kids[c] * 6);
-                    if (area > best) {
-                        best = area;
-                        pick = c;
-                    }
-                }
-                if (pick < 0) break;
-                const int inner = kids[pick];
-                kids[pick] = sc.left[inner];
-                kids[nk++] = sc.right[inner];
-            }
-            float cmin[kBVHWidth][3], cmax[kBVHWidth][3];
-            for (int c = 0; c < nk; c++) {
-                const float *b = kids[c] >= 0 ? sc.nodeBox + kids[c] * 6 : sc.leafBox + (~kids[c]) * 6;
-                for (int a = 0; a < 3; a++) {
-                    cmin[c][a] = b[a];
-                    cmax[c][a] = b[3 + a];
-                }
-            }
-            QBVHNode node;
-            quantizeNode(node, nk, cmin, cmax);
-            for (int c = 0; c < nk; c++) {
-                node.triSize[c] = 0;
-                if (kids[c] < 0) {
-                    node.childrenIdx[c] = 0x80000000u | (u32)sc.order[~kids[c]];
-                } else {
-                    const int id = atomicAdd(&sc.flags[0], 1);
-                    sc.wideBin[id] = (short)kids[c];
-                    sc.flags[id] = level + 1;
-                    depth = max(depth, level + 1);
-                    node.childrenIdx[c] = (u32)id;
-                }
-            }
-            out[k] = node;
+            const int nk = expandWide(kids, sc.wideBin[k], children, box);
+            writeWideNode(out + k, kids, nk, box, gatherIndex, [&](int bin) {
+                const int id = atomicAdd(&sc.flags[0], 1);
+                sc.wideBin[id] = (short)bin;
+                sc.flags[id] = level + 1;
+                depth = max(depth, level + 1);
+                return id;
+            });
         }
         __syncwarp();
         done = min(done + 32, count_now);
@@ -732,10 +780,10 @@ __device__ void blockSortKeys(unsigned long long *g, int n, unsigned long long *
 }
 
 // One block per world, worlds taken by ticket from the scan's list (a step without large
-// worlds costs one launch of blocks that find the list empty).  Same rules as the warp
-// builder, so the same tree: bounds of the box centres, Morton key << 32 | gather index,
-// Karras' split over the sorted keys, bottom-up boxes with arrival counters, 4-wide collapse
-// expanding the inner child of largest area (first maximum wins), quantizeNode.
+// worlds costs one launch of blocks that find the list empty).  The build rules are the shared
+// functions above, so the tree is renderBuildTLASKernel's; what is this kernel's own is the
+// bitonic sort, the scratch in global memory (TLASBuildNode) with __threadfence and __ldcg
+// reads of what other threads wrote, and the block-wide wave counter.
 __global__ void __launch_bounds__(kLargeTLASThreads)
 renderBuildLargeTLASKernel(EngineState *Sp)
 {
@@ -760,21 +808,9 @@ renderBuildLargeTLASKernel(EngineState *Sp)
         TLASBuildNode *bn = R.tlasBuild + offset;
         QBVHNode *out = R.tlasNodes + offset;
 
-        // 1. bounds of the box centres, Morton keys
-        float lo[3] = { FLT_MAX, FLT_MAX, FLT_MAX }, hi[3] = { -FLT_MAX, -FLT_MAX, -FLT_MAX };
-        for (int i = threadIdx.x; i < n; i += blockDim.x) {
-            for (int a = 0; a < 3; a++) {
-                const float c = 0.5f * (inst[i].aabbMin[a] + inst[i].aabbMax[a]);
-                lo[a] = fminf(lo[a], c);
-                hi[a] = fmaxf(hi[a], c);
-            }
-        }
-        for (int o = 16; o >= 1; o >>= 1) {
-            for (int a = 0; a < 3; a++) {
-                lo[a] = fminf(lo[a], __shfl_xor_sync(0xffffffffu, lo[a], o));
-                hi[a] = fmaxf(hi[a], __shfl_xor_sync(0xffffffffu, hi[a], o));
-            }
-        }
+        // 1. bounds of the box centres (the warps' combined through s_bounds), Morton keys
+        float lo[3], hi[3];
+        centreBounds(inst, n, threadIdx.x, blockDim.x, lo, hi);
         if (lane == 0) {
             for (int a = 0; a < 3; a++) {
                 s_bounds[a][warp] = lo[a];
@@ -790,48 +826,20 @@ renderBuildLargeTLASKernel(EngineState *Sp)
                 hi[a] = fmaxf(hi[a], s_bounds[3 + a][k]);
             }
         }
-        for (int i = threadIdx.x; i < n; i += blockDim.x) {
-            u32 code = 0;
-            for (int a = 0; a < 3; a++) {
-                const float c = 0.5f * (inst[i].aabbMin[a] + inst[i].aabbMax[a]);
-                const float ext = hi[a] - lo[a];
-                float u = ext > 0.f ? (c - lo[a]) / ext : 0.f;
-                u = fminf(fmaxf(u * 1024.f, 0.f), 1023.f);
-                code |= expandBits10((u32)u) << a;
-            }
-            keys[i] = ((unsigned long long)code << 32) | (u32)i;
-        }
+        for (int i = threadIdx.x; i < n; i += blockDim.x) keys[i] = mortonKey(inst[i], (u32)i, lo, hi);
         __syncthreads();
 
         // 2. sort; the low word of a sorted key is the instance's gather index
         blockSortKeys(keys, n, s_keys);
 
-        // 3. Karras 2012 over the sorted keys
+        // 3. internal nodes and parents
         for (int i = threadIdx.x; i < n - 1; i += blockDim.x) {
-            const int d = commonPrefix(keys, n, i, i + 1) - commonPrefix(keys, n, i, i - 1) >= 0 ? 1 : -1;
-            const int delta_min = commonPrefix(keys, n, i, i - d);
-            int lmax = 2;
-            while (commonPrefix(keys, n, i, i + lmax * d) > delta_min) lmax <<= 1;
-            int l = 0;
-            for (int t = lmax >> 1; t >= 1; t >>= 1) {
-                if (commonPrefix(keys, n, i, i + (l + t) * d) > delta_min) l += t;
-            }
-            const int j = i + l * d;
-            const int delta_node = commonPrefix(keys, n, i, j);
-            int s = 0;
-            for (int t = (l + 1) >> 1; ; t = (t + 1) >> 1) {
-                if (commonPrefix(keys, n, i, i + (s + t) * d) > delta_node) s += t;
-                if (t == 1) break;
-            }
-            const int gamma = i + s * d + min(d, 0);
-            const int first = min(i, j), last = max(i, j);
-            const int lc = first == gamma ? ~gamma : gamma;
-            const int rc = last == gamma + 1 ? ~(gamma + 1) : gamma + 1;
-            bn[i].left = lc;
-            bn[i].right = rc;
+            const int2 c = karrasSplit(keys, n, i);
+            bn[i].left = c.x;
+            bn[i].right = c.y;
             bn[i].arrivals = 0;
-            if (lc >= 0) bn[lc].parent = i; else bn[~lc].leafParent = i;
-            if (rc >= 0) bn[rc].parent = i; else bn[~rc].leafParent = i;
+            if (c.x >= 0) bn[c.x].parent = i; else bn[~c.x].leafParent = i;
+            if (c.y >= 0) bn[c.y].parent = i; else bn[~c.y].leafParent = i;
         }
         if (threadIdx.x == 0) bn[0].parent = -1;
         __syncthreads();
@@ -842,19 +850,14 @@ renderBuildLargeTLASKernel(EngineState *Sp)
             const RenderInstance &ri = inst[(u32)keys[pos]];
             return a < 3 ? ri.aabbMin[a] : ri.aabbMax[a - 3];
         };
+        auto l2Box = [&](int c, int a) { return c >= 0 ? __ldcg(&bn[c].box[a]) : leafBox(~c, a); };
         for (int leaf = threadIdx.x; leaf < n; leaf += blockDim.x) {
             int node = bn[leaf].leafParent;
             while (node >= 0) {
                 __threadfence();
                 if (atomicAdd(&bn[node].arrivals, 1) == 0) break;
                 const int lc = __ldcg(&bn[node].left), rc = __ldcg(&bn[node].right);
-                float b[6];
-                for (int a = 0; a < 6; a++) {
-                    const float lv = lc >= 0 ? __ldcg(&bn[lc].box[a]) : leafBox(~lc, a);
-                    const float rv = rc >= 0 ? __ldcg(&bn[rc].box[a]) : leafBox(~rc, a);
-                    b[a] = a < 3 ? fminf(lv, rv) : fmaxf(lv, rv);
-                }
-                for (int a = 0; a < 6; a++) bn[node].box[a] = b[a];
+                mergeBoxes(bn[node].box, lc, rc, l2Box);
                 node = __ldcg(&bn[node].parent);
             }
         }
@@ -869,55 +872,23 @@ renderBuildLargeTLASKernel(EngineState *Sp)
             s_depth = 1;
         }
         __syncthreads();
+        auto box = [&](int c, int a) { return c >= 0 ? bn[c].box[a] : leafBox(~c, a); };
+        auto children = [&](int b) { return make_int2(bn[b].left, bn[b].right); };
         for (int done = 0;;) {
             const int count_now = s_count;
             __syncthreads();
             if (done >= count_now) break;
             for (int k = done + threadIdx.x; k < count_now; k += blockDim.x) {
-                const int bin = bn[k].wideBin;
                 const int level = bn[k].wideDepth;
                 int kids[kBVHWidth];
-                int nk = 2;
-                kids[0] = bn[bin].left;
-                kids[1] = bn[bin].right;
-                while (nk < kBVHWidth) {
-                    int pick = -1;
-                    float best = -1.f;
-                    for (int c = 0; c < nk; c++) {
-                        if (kids[c] < 0) continue;
-                        const float area = wideChildArea(bn[kids[c]].box);
-                        if (area > best) {
-                            best = area;
-                            pick = c;
-                        }
-                    }
-                    if (pick < 0) break;
-                    const int inner = kids[pick];
-                    kids[pick] = bn[inner].left;
-                    kids[nk++] = bn[inner].right;
-                }
-                float cmin[kBVHWidth][3], cmax[kBVHWidth][3];
-                for (int c = 0; c < nk; c++) {
-                    for (int a = 0; a < 3; a++) {
-                        cmin[c][a] = kids[c] >= 0 ? bn[kids[c]].box[a] : leafBox(~kids[c], a);
-                        cmax[c][a] = kids[c] >= 0 ? bn[kids[c]].box[3 + a] : leafBox(~kids[c], 3 + a);
-                    }
-                }
-                QBVHNode node;
-                quantizeNode(node, nk, cmin, cmax);
-                for (int c = 0; c < nk; c++) {
-                    node.triSize[c] = 0;
-                    if (kids[c] < 0) {
-                        node.childrenIdx[c] = 0x80000000u | (u32)keys[~kids[c]];
-                    } else {
-                        const int id = atomicAdd(&s_count, 1);
-                        bn[id].wideBin = kids[c];
-                        bn[id].wideDepth = level + 1;
-                        atomicMax(&s_depth, level + 1);
-                        node.childrenIdx[c] = (u32)id;
-                    }
-                }
-                out[k] = node;
+                const int nk = expandWide(kids, bn[k].wideBin, children, box);
+                writeWideNode(out + k, kids, nk, box, [&](int pos) { return (u32)keys[pos]; }, [&](int bin) {
+                    const int id = atomicAdd(&s_count, 1);
+                    bn[id].wideBin = bin;
+                    bn[id].wideDepth = level + 1;
+                    atomicMax(&s_depth, level + 1);
+                    return id;
+                });
             }
             __syncthreads();
             done = count_now;
@@ -1698,8 +1669,7 @@ bool renderHostAfterRegistry(Executor *ex, std::string *err)
     // the output table may grow (during world construction or between steps): the view
     // list covers every row it can ever have, so no view is left unrendered
     R.maxViews = (i32)ex->maxRows[R.outputArchetype];
-    rh->tlasSmem = tlasScratchBytes(kWarpTLASInstances);
-    cudaFuncSetAttribute(renderBuildTLASKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rh->tlasSmem);
+    cudaFuncSetAttribute(renderBuildTLASKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTLASScratchBytes);
 
     // light carriers: archetypes with LightCarrier + Position + every LightDesc* component
     // (component ids are consecutive from registration: LightDesc, Direction, Type, Shadow,
@@ -1828,7 +1798,7 @@ bool renderEnqueuePrepare(Executor *ex, cudaStream_t s, std::string *err)
     }
     dim3 grid((unsigned)std::min((max_cap + 255) / 256, ex->numSMs * 4), std::max(R.numViewArchetypes, 1u));
     renderGatherViewsKernel<<<grid, 256, 0, s>>>(ex->dState);
-    renderBuildTLASKernel<<<W, 32, rh->tlasSmem, s>>>(ex->dState);
+    renderBuildTLASKernel<<<W, 32, kTLASScratchBytes, s>>>(ex->dState);
     // the step graph is captured once: the large-world builder's grid cannot follow the
     // per-step count, so its blocks take worlds by ticket and leave when the list is empty
     // (one block per SM: at 84 registers a second 512-thread block is not resident)

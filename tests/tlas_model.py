@@ -1,14 +1,18 @@
-"""numpy restatement of the ray caster's per-world TLAS build (kernels_render.cu:
-renderBuildTLASKernel for worlds of up to 128 instances, renderBuildLargeTLASKernel
-above), in float32 where the kernels use float32:
+"""numpy restatement of the ray caster's per-world TLAS build (kernels_render.cu), in
+float32 where the kernels use float32.  renderBuildTLASKernel (worlds of up to 128
+instances) and renderBuildLargeTLASKernel (above) both call one device function per rule,
+named after each rule below:
 
-  1. bounds of the instance box centres, 10-bit-per-axis Morton code of each centre,
-     key = morton << 32 | gather index (keys are unique, so the sorted order is unique);
-  2. Karras' split over the sorted keys, delta = -1 outside the world's segment;
-  3. bottom-up boxes (min / max: independent of the order nodes are finished in);
+  1. bounds of the instance box centres (centreBounds), 10-bit-per-axis Morton code of
+     each centre, key = morton << 32 | gather index (mortonKey; keys are unique, so the
+     sorted order is unique);
+  2. Karras' split over the sorted keys, delta = -1 outside the world's segment
+     (karrasSplit);
+  3. bottom-up boxes (mergeBoxes; min / max: independent of the order nodes are finished in);
   4. breadth-first collapse to 4-wide nodes: a node starts with its binary children and
-     repeatedly expands the inner child with the largest surface area (first maximum wins);
-  5. quantizeNode (render_bvh.h).
+     repeatedly expands the inner child with the largest surface area (expandWide,
+     wideChildArea; first maximum wins);
+  5. quantizeNode (render_bvh.h) and the child encoding (writeWideNode).
 
 build_tlas() returns the tree canonicalised depth-first from the root with children in
 slot order, so it can be compared byte for byte with the engine's nodes after the same
@@ -55,7 +59,7 @@ def _fma(a, b, c):
 
 
 def child_area(lo, hi):
-    """wideChildArea(): dx*dy + dy*dz + dz*dx as the kernels evaluate it (fmas spelled out)."""
+    """wideChildArea(): dx*dy + dy*dz + dz*dx as the kernel evaluates it (fmas spelled out)."""
     dx, dy, dz = F32(hi[0] - lo[0]), F32(hi[1] - lo[1]), F32(hi[2] - lo[2])
     return _fma(dx, dz, _fma(dx, dy, F32(dy * dz)))
 
