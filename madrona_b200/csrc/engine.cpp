@@ -370,6 +370,16 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
         }
     }
 
+    {
+        // so is the hull-size knob of the physics narrowphase
+        int max_hull_size;
+        std::string err;
+        if (!physicsMaxHullSize(&max_hull_size, &err)) {
+            setError(err);
+            return false;
+        }
+    }
+
     MB2_CUDA(cudaSetDevice(ex->gpu));
     cudaDeviceProp prop;
     MB2_CUDA(cudaGetDeviceProperties(&prop, ex->gpu));

@@ -79,6 +79,13 @@ struct PhysicsHost {
     bool active = false;
     bool spheres = false;     // some registered object has a sphere primitive (read before graph capture)
     unsigned narrowBlocks = 0;   // persistent narrowphase grid for that kernel (0: occupancy query failed)
+    // hulls past the staging caps (MADRONA_B200_MAX_HULL_SIZE > 16)
+    i32 *classInfo = nullptr;        // device scratch of the primitive classification
+    unsigned char *primClass = nullptr;
+    i32 primClassCapacity = 0;
+    bool largeHulls = false;         // some primitive needs the warp-per-pair kernel (read before graph capture)
+    unsigned largeBlocks = 0;        // its persistent grid (0: it does not fit / the query failed)
+    std::string largeError;          // why a launch graph with physics cannot be built
 };
 
 // ---- small device helpers ------------------------------------------------------------
@@ -689,12 +696,31 @@ __device__ void phaseFindCandidates(EngineState &S, const PhysicsState &P, const
     }
     if (lane == 0) P.candCounts[w] = running;
 
-    // the step's two work lists, hull - hull pairs and the others (one atomic per
-    // warp, list and 32 candidates)
+    // the step's work lists, hull - hull pairs and the others (one atomic per warp, list
+    // and 32 candidates); with a primitive class table, the pairs of any type that have a
+    // hull past the staging caps go to a third list instead
     __syncwarp();
+    const unsigned char *const prim_class = P.primClass;     // uniform for the launch
     for (i32 base = 0; base < running; base += 32) {
         const i32 i = base + lane;
-        const bool valid = i < running;
+        bool valid = i < running;
+        if (prim_class) {
+            bool large = false;
+            if (valid) {
+                const u32 pa = out[i].aPrim, pb = out[i].bPrim;
+                const u32 n = (u32)P.numPrimClasses;
+                large = (pa < n ? prim_class[pa] : (u32)PrimTooLarge) != PrimSmall ||
+                        (pb < n ? prim_class[pb] : (u32)PrimTooLarge) != PrimSmall;
+            }
+            const unsigned large_mask = __ballot_sync(0xffffffffu, large);
+            if (large_mask) {
+                i32 large_at = 0;
+                if (lane == 0) large_at = atomicAdd(&P.largeCounts[0], __popc(large_mask));
+                large_at = __shfl_sync(0xffffffffu, large_at, 0);
+                if (large) P.largePairs[large_at + __popc(large_mask & ((1u << lane) - 1u))] = PairEntry { w, i };
+                valid = valid && !large;
+            }
+        }
         const bool hh = valid && (out[i].arch >> 16) == 2u;
         const unsigned hh_mask = __ballot_sync(0xffffffffu, hh);
         const unsigned other_mask = __ballot_sync(0xffffffffu, valid && !hh);
@@ -1116,11 +1142,36 @@ struct HullScratch {
     float depths[kClipCap];
 };
 
+// Where the group of a hull - hull pair stages both hulls, the clipped polygon and its
+// depths, and how much fits: the HullScratch of an 8-lane group, or a warp's slice of
+// dynamic shared memory sized from PhysicsState::maxHullSize (physNarrowphaseLargeKernel).
+struct HullStage {
+    Vector3 *vertsA, *vertsB;
+    Plane *planesA, *planesB;
+    Vector3 *clipA, *clipB;     // clipCap points each
+    float *depths;              // clipCap
+    int maxVerts, maxFaces, maxFaceVerts, clipCap;
+};
+
+__device__ __forceinline__ HullStage smallHullStage(HullScratch &s)
+{
+    return HullStage { s.verts, s.verts + kMaxHullVerts, s.planes, s.planes + kMaxHullFaces,
+                       s.clipA, s.clipB, s.depths, kMaxHullVerts, kMaxHullFaces, kMaxFaceVerts, kClipCap };
+}
+
 // hull - plane pairs: the incident face's points and what groupManifold keeps of them
 struct PlaneScratch {
     Vector3 pts[kMaxFaceVerts];
     Vector3 kept[kMaxFaceVerts];
     float depths[kMaxFaceVerts];
+    static constexpr int cap = kMaxFaceVerts;
+};
+
+// the same in a warp's slice of dynamic shared memory (physNarrowphaseLargeKernel)
+struct LargePlaneStage {
+    Vector3 *pts, *kept;
+    float *depths;
+    int cap;
 };
 
 // (value, index) of the element a sequential scan would have kept.
@@ -1133,14 +1184,16 @@ struct Winner {
 // aligned group).  Input per lane: its own candidate (sep, idx) chosen by the
 // same rule over the elements it looked at, or have = false.
 // Rule == the scalar loop "keep strictly greater, stop at the first positive":
-// lowest index among positives, else lowest index among maxima.
+// lowest index among positives, else lowest index among maxima -- for any number of lanes
+// G the elements were dealt to.
+template <int G = kGroupLanes>
 __device__ __forceinline__ Winner groupSequentialWinner(unsigned gm, float sep, i32 idx, bool have)
 {
     const bool positive = have && sep > 0.f;
     if (__any_sync(gm, positive)) {
         i32 cand = positive ? idx : 0x7fffffff;
 #pragma unroll
-        for (int o = kGroupLanes / 2; o >= 1; o >>= 1) {
+        for (int o = G / 2; o >= 1; o >>= 1) {
             const i32 other = __shfl_xor_sync(gm, cand, o);
             if (other < cand) cand = other;
         }
@@ -1151,7 +1204,7 @@ __device__ __forceinline__ Winner groupSequentialWinner(unsigned gm, float sep, 
     float s = have ? sep : -FLT_MAX;
     i32 k = have ? idx : 0x7fffffff;
 #pragma unroll
-    for (int o = kGroupLanes / 2; o >= 1; o >>= 1) {
+    for (int o = G / 2; o >= 1; o >>= 1) {
         const float os = __shfl_xor_sync(gm, s, o);
         const i32 ok = __shfl_xor_sync(gm, k, o);
         if (os > s || (os == s && ok < k)) {
@@ -1184,13 +1237,14 @@ __device__ __forceinline__ Winner groupFirstBest(unsigned gm, float v, i32 idx, 
 }
 
 // face of a hull most anti-parallel to the reference normal, first minimum wins
+template <int G = kGroupLanes>
 __device__ __forceinline__ i32 groupMostOpposedFace(unsigned gm, int sub, const Plane *planes, u32 num_faces,
                                                     Vector3 ref_normal)
 {
     float lowest = FLT_MAX;
     i32 face = 0;
     bool have = false;
-    for (u32 f = (u32)sub; f < num_faces; f += kGroupLanes) {
+    for (u32 f = (u32)sub; f < num_faces; f += G) {
         const float d = dot(planes[f].normal, ref_normal);
         if (d < lowest) {
             lowest = d;
@@ -1198,7 +1252,7 @@ __device__ __forceinline__ i32 groupMostOpposedFace(unsigned gm, int sub, const 
             have = true;
         }
     }
-    return groupFirstBest<true>(gm, lowest, face, have).idx;
+    return groupFirstBest<true, G>(gm, lowest, face, have).idx;
 }
 
 // Keep the points pts[0, n) at or below the reference plane, projected onto it with
@@ -1309,9 +1363,9 @@ __device__ int groupManifold(unsigned gm, int sub, const Plane &ref_plane, const
 // hull (a) - plane (b, the reference).  The hull is never stored: each lane places
 // the vertices and face normals it reads (vertex = R S v + t, normal =
 // normalize(R S^-1 n)).  Returns, on every lane of the group, whether a contact
-// was written to `out`.
-template <int G>
-__device__ bool hullPlaneGroup(EngineState &S, const PairSetup &ps, PlaneScratch &scratch, const unsigned gm,
+// was written to `out`.  Stage: PlaneScratch or LargePlaneStage.
+template <int G, typename Stage>
+__device__ bool hullPlaneGroup(EngineState &S, const PairSetup &ps, Stage &scratch, const unsigned gm,
                                const int sub, Contact &out)
 {
     const HalfEdgeMesh &am = ps.aPrim->hull;
@@ -1356,10 +1410,10 @@ __device__ bool hullPlaneGroup(EngineState &S, const PairSetup &ps, PlaneScratch
     do {
         const HalfEdge cur = am.halfEdges[he];
         he = cur.next;
-        if (nv < kMaxFaceVerts && nv % G == sub) scratch.pts[nv] = vert_m * am.vertices[cur.rootVertex] + ps.aPos;
+        if (nv < scratch.cap && nv % G == sub) scratch.pts[nv] = vert_m * am.vertices[cur.rootVertex] + ps.aPos;
         nv++;
-    } while (he != start && nv <= kMaxFaceVerts);
-    if (nv > kMaxFaceVerts) {
+    } while (he != start && nv <= scratch.cap);
+    if (nv > scratch.cap) {
         if (sub == 0) atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
         return false;
     }
@@ -1371,15 +1425,16 @@ __device__ bool hullPlaneGroup(EngineState &S, const PairSetup &ps, PlaneScratch
 }
 
 // faces of one hull against the other hull's vertices: lane `sub` measures faces
-// sub, sub + 8, ... in ascending order with the scalar rule, then the group combines
+// sub, sub + G, ... in ascending order with the scalar rule, then the group combines
 // (narrowphase.cpp:339-365)
+template <int G = kGroupLanes>
 __device__ __forceinline__ Winner groupFaceQuery(unsigned gm, int sub, const Plane *planes, u32 num_faces,
                                                  const Vector3 *other_verts, u32 other_num_verts)
 {
     float best = -FLT_MAX;
     i32 best_face = 0x7fffffff;
     bool have = false;
-    for (u32 f = (u32)sub; f < num_faces; f += kGroupLanes) {
+    for (u32 f = (u32)sub; f < num_faces; f += G) {
         const Plane pl = planes[f];
         float lowest = FLT_MAX;
 #pragma unroll 1
@@ -1396,40 +1451,41 @@ __device__ __forceinline__ Winner groupFaceQuery(unsigned gm, int sub, const Pla
             if (sep > 0.f) break;    // the scalar loop stops at the first positive
         }
     }
-    return groupSequentialWinner(gm, best, best_face, have);
+    return groupSequentialWinner<G>(gm, best, best_face, have);
 }
 
-// Executed by the kGroupLanes lanes of one group for the hull - hull pair `ps`
-// (every lane holds the same copy).  Returns, on every lane of the group, whether
+// Executed by the G lanes of one group for the hull - hull pair `ps` (every lane
+// holds the same copy), staging in `st`.  Returns, on every lane of the group, whether
 // a contact was written to `out`.
-__device__ bool hullHullGroup(EngineState &S, const PairSetup &ps, HullScratch &scratch, const unsigned gm,
+template <int G>
+__device__ bool hullHullGroup(EngineState &S, const PairSetup &ps, const HullStage &st, const unsigned gm,
                               const int sub, Contact &out)
 {
     const HalfEdgeMesh &am = ps.aPrim->hull;
     const HalfEdgeMesh &bm = ps.bPrim->hull;
     const u32 nva = am.numVertices, nvb = bm.numVertices, nfa = am.numFaces, nfb = bm.numFaces;
-    if (nva > (u32)kMaxHullVerts || nvb > (u32)kMaxHullVerts ||
-            nfa > (u32)kMaxHullFaces || nfb > (u32)kMaxHullFaces) {
+    if (nva > (u32)st.maxVerts || nvb > (u32)st.maxVerts ||
+            nfa > (u32)st.maxFaces || nfb > (u32)st.maxFaces) {
         if (sub == 0) atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
         return false;
     }
 
     // -- both hulls into shared memory (vertex = R S v + t, plane via R S^-1,
     // plane offset through a transformed point of the plane: narrowphase.cpp:151-223)
-    Vector3 *verts_a = scratch.verts, *verts_b = scratch.verts + kMaxHullVerts;
-    Plane *planes_a = scratch.planes, *planes_b = scratch.planes + kMaxHullFaces;
+    Vector3 *verts_a = st.vertsA, *verts_b = st.vertsB;
+    Plane *planes_a = st.planesA, *planes_b = st.planesB;
     {
         const Mat3x3 rot_a = Mat3x3::fromQuat(ps.aRot), rot_b = Mat3x3::fromQuat(ps.bRot);
         const Mat3x3 vm_a = rot_a * ps.aScale, vm_b = rot_b * ps.bScale;
         const Mat3x3 nm_a = rot_a * ps.aScale.inv(), nm_b = rot_b * ps.bScale.inv();
         const Vector3 a_pos = ps.aPos, b_pos = ps.bPos;
 #pragma unroll 1
-        for (u32 i = (u32)sub; i < nva + nvb; i += kGroupLanes) {
+        for (u32 i = (u32)sub; i < nva + nvb; i += G) {
             if (i < nva) verts_a[i] = vm_a * am.vertices[i] + a_pos;
             else verts_b[i - nva] = vm_b * bm.vertices[i - nva] + b_pos;
         }
 #pragma unroll 1
-        for (u32 i = (u32)sub; i < nfa + nfb; i += kGroupLanes) {
+        for (u32 i = (u32)sub; i < nfa + nfb; i += G) {
             const bool is_a = i < nfa;
             const Plane local = is_a ? am.facePlanes[i] : bm.facePlanes[i - nfa];
             const Mat3x3 vm = is_a ? vm_a : vm_b;    // by value: a reference would put both in local memory
@@ -1447,22 +1503,22 @@ __device__ bool hullHullGroup(EngineState &S, const PairSetup &ps, HullScratch &
     center_a /= (float)nva;
 
     // -- face queries (A's faces vs B, then B's vs A)
-    const Winner fa = groupFaceQuery(gm, sub, planes_a, nfa, verts_b, nvb);
+    const Winner fa = groupFaceQuery<G>(gm, sub, planes_a, nfa, verts_b, nvb);
     if (fa.sep > 0.0f) return false;
-    const Winner fb = groupFaceQuery(gm, sub, planes_b, nfb, verts_a, nva);
+    const Winner fb = groupFaceQuery<G>(gm, sub, planes_b, nfb, verts_a, nva);
     if (fb.sep > 0.0f) return false;
     const float sep_a = fa.sep, sep_b = fb.sep;
     const i32 face_a = fa.idx, face_b = fb.idx;
 
     // -- edge query: edge pairs a-major over numHalfEdges/2 edges (half-edge 2k, twin
     // 2k+1), only pairs forming a face of the Minkowski difference are measured
-    // (narrowphase.cpp:367-567); pair p = ia * eb + ib, lanes take p = sub, sub + 8, ...
+    // (narrowphase.cpp:367-567); pair p = ia * eb + ib, lanes take p = sub, sub + G, ...
     const u32 ea = am.numHalfEdges / 2, eb = bm.numHalfEdges / 2;
     float e_sep = -FLT_MAX;
     i32 e_pair = 0x7fffffff;
     Vector3 e_normal = Vector3::zero();
 #pragma unroll 1
-    for (u32 p = (u32)sub; p < ea * eb; p += kGroupLanes) {
+    for (u32 p = (u32)sub; p < ea * eb; p += G) {
         const u32 ha = (p / eb) * 2, hb = (p % eb) * 2;
         const HalfEdge a0 = am.halfEdges[ha];
         const HalfEdge a1 = am.halfEdges[ha ^ 1u];
@@ -1494,7 +1550,7 @@ __device__ bool hullHullGroup(EngineState &S, const PairSetup &ps, HullScratch &
     {
         const float my_sep = e_sep;
         const i32 my_pair = e_pair;
-        const Winner ew = groupSequentialWinner(gm, e_sep, e_pair, my_pair != 0x7fffffff);
+        const Winner ew = groupSequentialWinner<G>(gm, e_sep, e_pair, my_pair != 0x7fffffff);
         e_sep = ew.sep;
         e_pair = ew.idx;
         const unsigned owner = __ballot_sync(gm, my_pair == e_pair && my_pair != 0x7fffffff &&
@@ -1537,23 +1593,23 @@ __device__ bool hullHullGroup(EngineState &S, const PairSetup &ps, HullScratch &
     const HalfEdgeMesh &inc_mesh = a_is_ref ? bm : am;
     const Vector3 *ref_verts = a_is_ref ? verts_a : verts_b;
     const Vector3 *inc_verts = a_is_ref ? verts_b : verts_a;
-    const i32 inc_face = groupMostOpposedFace(gm, sub, a_is_ref ? planes_b : planes_a, a_is_ref ? nfb : nfa,
-                                              ref_plane.normal);
+    const i32 inc_face = groupMostOpposedFace<G>(gm, sub, a_is_ref ? planes_b : planes_a, a_is_ref ? nfb : nfa,
+                                                 ref_plane.normal);
     if (inc_face == 0x7fffffff) return false;
 
     // incident polygon clipped against the side planes of the reference face
     // (normal = edge x n_ref), on the group's first lane; result in clipA (0) or clipB (1).
-    // Either face over kMaxFaceVerts vertices, or a clipped polygon over kClipCap points
+    // Either face over st.maxFaceVerts vertices, or a clipped polygon over st.clipCap points
     // (k-gon against k-gon: up to 2k), is an overflow: n = -1, and no contact.
     int n = 0, in_b = 0;
     if (sub == 0) {
-        Vector3 *src = scratch.clipA, *dst = scratch.clipB;
+        Vector3 *src = st.clipA, *dst = st.clipB;
         u32 he = inc_mesh.faceBaseHalfEdges[inc_face];
         u32 start = he;
         do {
             const HalfEdge cur = inc_mesh.halfEdges[he];
             he = cur.next;
-            if (n == kMaxFaceVerts) {
+            if (n == st.maxFaceVerts) {
                 n = -1;
                 break;
             }
@@ -1564,7 +1620,7 @@ __device__ bool hullHullGroup(EngineState &S, const PairSetup &ps, HullScratch &
         Vector3 cur_pt = ref_verts[ref_mesh.halfEdges[he].rootVertex];
         int sides = 0;
         while (n >= 0) {
-            if (++sides > kMaxFaceVerts) {
+            if (++sides > st.maxFaceVerts) {
                 n = -1;
                 break;
             }
@@ -1573,7 +1629,7 @@ __device__ bool hullHullGroup(EngineState &S, const PairSetup &ps, HullScratch &
             Vector3 side_n = cross(next_pt - cur_pt, ref_plane.normal);
             Plane side { side_n, dot(side_n, cur_pt) };
             cur_pt = next_pt;
-            if (n > 0) n = clipAgainst(dst, side, src, n, kClipCap);
+            if (n > 0) n = clipAgainst(dst, side, src, n, st.clipCap);
             Vector3 *tmp = src;
             src = dst;
             dst = tmp;
@@ -1587,8 +1643,8 @@ __device__ bool hullHullGroup(EngineState &S, const PairSetup &ps, HullScratch &
     if (n < 0) return false;
     in_b = __shfl_sync(gm, in_b, leader);
     __syncwarp(gm);
-    const int count = groupManifold<kGroupLanes>(gm, sub, ref_plane, in_b ? scratch.clipB : scratch.clipA, n,
-                                    in_b ? scratch.clipA : scratch.clipB, scratch.depths, out);
+    const int count = groupManifold<G>(gm, sub, ref_plane, in_b ? st.clipB : st.clipA, n,
+                                       in_b ? st.clipA : st.clipB, st.depths, out);
     if (count == 0) return false;
     if (sub == 0) {
         if (a_is_ref) writeContactHeader(out, ps.aArch, ps.aRow, ps.aInfo, ps.bArch, ps.bRow, ps.bInfo, count, ref_plane.normal);
@@ -1663,8 +1719,8 @@ physNarrowphaseKernel(EngineState *Sp)
             const PairEntry ent = P.hullPairs[e];
             const size_t slot = (size_t)ent.world * P.maxCandidatesPerWorld + ent.cand;
             const PairSetup ps = setupPair(worldObjects(S, P, ent.world), P.candidates[slot]);
-            const bool made = ps.test != 0 && hullHullGroup(S, ps, scratch[warp].hull[group], gm, sub,
-                                                             P.contacts[slot]);
+            const bool made = ps.test != 0 && hullHullGroup<kGroupLanes>(
+                S, ps, smallHullStage(scratch[warp].hull[group]), gm, sub, P.contacts[slot]);
             if (sub == 0) P.candHit[slot] = made ? 1 : 0;
         }
         // the warp's next item may use its scratch in the other layout
@@ -1701,6 +1757,213 @@ physNarrowphaseKernel(EngineState *Sp)
         P.pairCounts[2] = 0;
         P.pairCounts[3] = 0;
     }
+}
+
+// ---- hulls past the staging caps: one warp per pair --------------------------------------
+// With MADRONA_B200_MAX_HULL_SIZE = N > 16 and a primitive that needs it, the candidate
+// search sends every pair with such a hull to PhysicsState::largePairs and each substep
+// runs this kernel after the one above: the same group functions with all 32 lanes on one
+// pair (the winner rules do not depend on the lane count, so the results are the scalar
+// scan's), staging in dynamic shared memory sized from N instead of the fixed scratch --
+// per warp both hulls' planes and vertices (2N x 16 B, 2N x 12 B), two clip buffers of 2N
+// points and 2N depths: 112 N bytes, 3.5 KB at N = 32 and 27.9 KB at N = 255, where the 8
+// warps of a block fill an SM's shared memory.  (A convex polygon of n points clipped by m
+// side planes has at most n + m <= 2N; vertices that round onto a side plane can add a few,
+// tests/test_large_hull_model.py, so clipAgainst keeps its "would not fit" return.)  The grid is what is resident at that size; pairs are handed out
+// by a ticket as above, and each writes only its own contact slot and candHit entry.
+constexpr int kLargeWarps = 8;
+constexpr int kLargeThreads = 32 * kLargeWarps;
+constexpr int kLargeStageBytesPerEntry = 2 * (int)(sizeof(Plane) + 3 * sizeof(Vector3) + sizeof(float));
+static_assert(kLargeStageBytesPerEntry == 112, "large-hull stage layout");
+
+__device__ __forceinline__ HullStage largeHullStage(unsigned char *base, const int n)
+{
+    Plane *planes = (Plane *)base;
+    Vector3 *verts = (Vector3 *)(planes + 2 * n);
+    Vector3 *clip_a = verts + 2 * n, *clip_b = clip_a + 2 * n;
+    return HullStage { verts, verts + n, planes, planes + n, clip_a, clip_b, (float *)(clip_b + 2 * n),
+                       n, n, n, 2 * n };
+}
+
+// sphere (a) - hull (b) by one warp, the arithmetic of sphereHullContact: the translated
+// vertices are staged by all lanes, GJK runs on lane 0, the face scan of a centre inside
+// the hull is dealt to the lanes ("first strictly greater" == lowest index among maxima).
+// Lane 0 writes the contact; returns on every lane whether there is one.
+__device__ bool sphereHullWarp(const PairSetup &ps, const HullStage &st, const int lane, Contact &out)
+{
+    const HalfEdgeMesh &bm = ps.bPrim->hull;
+    const float radius = ps.aScale.d0 * ps.aPrim->sphereRadius;
+    const Vector3 a_pos = ps.aPos;
+    const Vector3 hull_origin = ps.bPos - a_pos;
+    const Mat3x3 rot = Mat3x3::fromQuat(ps.bRot);
+    const Mat3x3 vert_m = rot * ps.bScale;
+    const Mat3x3 norm_m = rot * ps.bScale.inv();
+    Vector3 *verts = st.vertsA;     // maxVerts entries: the caller checked the hull against it
+#pragma unroll 1
+    for (u32 i = (u32)lane; i < bm.numVertices; i += 32) verts[i] = vert_m * bm.vertices[i] + hull_origin;
+    __syncwarp();
+
+    Vector3 to_hull = Vector3::zero();
+    float dist2 = 0.f;
+    if (lane == 0) {
+        dist2 = madrona::geo::hullVerticesClosestPointToOriginGJK(verts, bm.numVertices, 1e-10f, &to_hull);
+    }
+    dist2 = __shfl_sync(0xffffffffu, dist2, 0);
+    if (dist2 > radius * radius) return false;
+
+    if (dist2 == 0.f) {
+        float best = -FLT_MAX;
+        i32 best_face = 0;
+        Vector3 best_n = Vector3::zero();
+        bool have = false;
+#pragma unroll 1
+        for (u32 f = (u32)lane; f < bm.numFaces; f += 32) {
+            const Plane local = bm.facePlanes[f];
+            const Vector3 on_plane = vert_m * (local.normal * local.d) + hull_origin;
+            const Vector3 n = (norm_m * local.normal).normalize();
+            const float face_dist = -dot(n, on_plane);
+            if (face_dist > best) {
+                best = face_dist;
+                best_face = (i32)f;
+                best_n = n;
+                have = true;
+            }
+        }
+        const Winner win = groupFirstBest<false, 32>(0xffffffffu, best, best_face, have);
+        // no face beat the scan's start value: it keeps -FLT_MAX and a zero normal
+        const float max_sep = win.idx == 0x7fffffff ? -FLT_MAX : win.sep;
+        if (max_sep > 0.f) return false;      // GJK and SAT disagree by rounding
+        const unsigned owner = __ballot_sync(0xffffffffu, have && best_face == win.idx);
+        if (owner && lane == __ffs(owner) - 1) {
+            writeSinglePointContact(out, ps.bArch, ps.bRow, ps.bInfo, ps.aArch, ps.aRow, ps.aInfo,
+                                    a_pos + best_n * radius, best_n, -max_sep);
+        } else if (!owner && lane == 0) {
+            const Vector3 zero = Vector3::zero();
+            writeSinglePointContact(out, ps.bArch, ps.bRow, ps.bInfo, ps.aArch, ps.aRow, ps.aInfo,
+                                    a_pos + zero * radius, zero, -max_sep);
+        }
+        return true;
+    }
+    if (lane == 0) {
+        const float to_hull_len = sqrtf(dist2);
+        const Vector3 normal = to_hull / to_hull_len;
+        writeSinglePointContact(out, ps.bArch, ps.bRow, ps.bInfo, ps.aArch, ps.aRow, ps.aInfo,
+                                a_pos + normal * radius, -normal, radius - to_hull_len);
+    }
+    return true;
+}
+
+__global__ void __launch_bounds__(kLargeThreads, 1)
+physNarrowphaseLargeKernel(EngineState *Sp)
+{
+    EngineState &S = *Sp;
+    const PhysicsState &P = *S.physics;
+    fillColCache(S, P);
+    extern __shared__ __align__(16) unsigned char large_stage[];
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x / 32;
+    const int cap = P.maxHullSize;
+    const HullStage st = largeHullStage(large_stage + (size_t)warp * cap * kLargeStageBytesPerEntry, cap);
+    const i32 num_pairs = P.largeCounts[0];
+    i32 *const ticket = &P.largeCounts[1];
+    i32 item = 0;
+    if (lane == 0) item = atomicAdd(ticket, 1);
+    item = __shfl_sync(0xffffffffu, item, 0);
+
+    while (item < num_pairs) {
+        i32 next = 0;
+        if (lane == 0) next = atomicAdd(ticket, 1);    // in flight while this pair runs
+        const PairEntry ent = P.largePairs[item];
+        const size_t slot = (size_t)ent.world * P.maxCandidatesPerWorld + ent.cand;
+        const PairSetup ps = setupPair(worldObjects(S, P, ent.world), P.candidates[slot]);
+        bool made = false;
+        if (ps.test != 0) {
+            // side a is a hull except in sphere - hull pairs, side b except in hull - plane pairs
+            const HalfEdgeMesh *ha = ps.test != 3 ? &ps.aPrim->hull : nullptr;
+            const HalfEdgeMesh *hb = ps.test != 6 ? &ps.bPrim->hull : nullptr;
+            const bool fits = (!ha || (ha->numVertices <= (u32)cap && ha->numFaces <= (u32)cap)) &&
+                              (!hb || (hb->numVertices <= (u32)cap && hb->numFaces <= (u32)cap));
+            if (!fits || (ps.test != 2 && ps.test != 3 && ps.test != 6)) {
+                if (lane == 0) atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
+            } else if (ps.test == 2) {
+                made = hullHullGroup<32>(S, ps, st, 0xffffffffu, lane, P.contacts[slot]);
+            } else if (ps.test == 6) {
+                LargePlaneStage plane_stage { st.clipA, st.clipB, st.depths, st.maxFaceVerts };
+                made = hullPlaneGroup<32>(S, ps, plane_stage, 0xffffffffu, lane, P.contacts[slot]);
+            } else {
+                made = sphereHullWarp(ps, st, lane, P.contacts[slot]);
+            }
+        }
+        if (lane == 0) P.candHit[slot] = made ? 1 : 0;
+        // the stage is reused by the warp's next pair
+        __syncwarp();
+        item = __shfl_sync(0xffffffffu, next, 0);
+    }
+    // as in physNarrowphaseKernel: the last warp out zeroes the ticket for the next launch
+    if (lane == 0 && atomicAdd(&P.largeCounts[2], 1) == (i32)gridDim.x * kLargeWarps - 1) {
+        P.largeCounts[1] = 0;
+        P.largeCounts[2] = 0;
+    }
+}
+
+// ---- primitive classes, once before the launch graph is captured --------------------------
+// The half-edge mesh does not store its largest face, so a primitive's class (PrimClass)
+// comes from a walk over its faces.  The ObjectManager carries no primitive count either:
+// physPrimExtentKernel takes it from the objects the bodies use, and checks that every
+// world points at the ObjectManager of world 0, whose primitives the table describes.
+// info[0] = primitives, info[1] = worlds with another ObjectManager, info[2] = primitives
+// that are not small.
+__global__ void __launch_bounds__(256)
+physPrimExtentKernel(EngineState *Sp, i32 *info)
+{
+    const EngineState &S = *Sp;
+    const PhysicsState &P = *S.physics;
+    const ObjectManager *first = &worldObjects(S, P, 0);
+    const i32 tid = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
+    for (i32 w = tid; w < (i32)S.numWorlds; w += stride) {
+        if (&worldObjects(S, P, w) != first) atomicAdd(&info[1], 1);
+    }
+    for (u32 bi = 0; bi < P.numBodyArchetypes; bi++) {
+        const BodyArchetype &b = P.bodies[bi];
+        const TableDesc &t = S.tables[b.archetype];
+        for (i32 row = tid; row < t.numRows; row += stride) {
+            if (((const i32 *)t.columns[1])[row] < 0) continue;
+            const i32 obj = bodyCol<i32>(S, b, PCObjectID, row);
+            atomicMax(&info[0], (i32)(first->primOffsets[obj] + first->primCounts[obj]));
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256)
+physClassifyPrimsKernel(EngineState *Sp, unsigned char *classes, i32 num_prims, i32 *info)
+{
+    const EngineState &S = *Sp;
+    const PhysicsState &P = *S.physics;
+    const i32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= num_prims) return;
+    const CollisionPrimitive &prim = worldObjects(S, P, 0).prims[i];
+    u32 cls = PrimSmall;
+    if (prim.type == 2u) {
+        const HalfEdgeMesh &m = prim.hull;
+        // the longest face loop; a walk is bounded by the mesh's half-edges, so a broken
+        // `next` chain cannot loop for ever (it then counts as a face of that length)
+        u32 longest = 0;
+        for (u32 f = 0; f < m.numFaces; f++) {
+            const u32 start = m.faceBaseHalfEdges[f];
+            u32 he = start, n = 0;
+            do {
+                he = m.halfEdges[he].next;
+                n++;
+            } while (he != start && he < m.numHalfEdges && n < m.numHalfEdges);
+            if (n > longest) longest = n;
+        }
+        const u32 cap = (u32)P.maxHullSize;
+        if (m.numVertices > cap || m.numFaces > cap || longest > cap) cls = PrimTooLarge;
+        else if (m.numVertices > (u32)kMaxHullVerts || m.numFaces > (u32)kMaxHullFaces ||
+                 longest > (u32)kMaxFaceVerts) cls = PrimLarge;
+    }
+    classes[i] = (unsigned char)cls;
+    if (cls != PrimSmall) atomicAdd(&info[2], 1);
 }
 
 // Prologue of the position solve, run by the LPW lanes that own world w: list
@@ -2556,6 +2819,27 @@ static uint64_t envU64p(const char *name, uint64_t dflt)
     return (v && *v) ? strtoull(v, nullptr, 10) : dflt;
 }
 
+bool physicsMaxHullSize(int *size, std::string *err)
+{
+    *size = kMinHullSizeCap;
+    const char *v = getenv("MADRONA_B200_MAX_HULL_SIZE");
+    if (!v || !*v) return true;
+    char *end = nullptr;
+    const long n = strtol(v, &end, 10);
+    if (*end != '\0' || n < kMinHullSizeCap || n > kMaxHullSizeCap) {
+        *err = "MADRONA_B200_MAX_HULL_SIZE must be a number from " + std::to_string(kMinHullSizeCap) + " to " +
+               std::to_string(kMaxHullSizeCap) + " (vertices and faces per convex hull), got \"" + v + "\"";
+        return false;
+    }
+    *size = (int)n;
+    return true;
+}
+
+static size_t largeStageBytes(int max_hull_size)
+{
+    return (size_t)kLargeWarps * max_hull_size * kLargeStageBytesPerEntry;
+}
+
 bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::string *err)
 {
     PhysicsHost *ph = ex->physics;
@@ -2613,6 +2897,24 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::stri
         *err = "physics buffers allocation failed";
         return false;
     }
+    // hulls past the staging caps: the third work list and its kernel's shared memory
+    int max_hull_size = kMinHullSizeCap;
+    if (!physicsMaxHullSize(&max_hull_size, err)) return false;
+    P.maxHullSize = max_hull_size;
+    if (max_hull_size > kMinHullSizeCap) {
+        if (!alloc((void **)&P.largePairs, sizeof(PairEntry) * W * P.maxCandidatesPerWorld) ||
+            !alloc((void **)&P.largeCounts, sizeof(i32) * 3) ||
+            !alloc((void **)&ph->classInfo, sizeof(i32) * 3)) {
+            *err = "physics buffers allocation failed";
+            return false;
+        }
+        if (cudaFuncSetAttribute(physNarrowphaseLargeKernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)largeStageBytes(max_hull_size)) != cudaSuccess) {
+            cudaGetLastError();
+            *err = "the large-hull narrowphase's shared memory (MADRONA_B200_MAX_HULL_SIZE) does not fit the device";
+            return false;
+        }
+    }
     cudaMemcpy(ph->dPhys, &P, sizeof(PhysicsState), cudaMemcpyHostToDevice);
     // the position solve's body stage: prefer shared memory over L1 (measured with this setting)
     if (cudaFuncSetAttribute(physSolvePositionsKernel, cudaFuncAttributePreferredSharedMemoryCarveout,
@@ -2621,6 +2923,59 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::stri
         return false;
     }
     return true;
+}
+
+// MADRONA_B200_MAX_HULL_SIZE > 16: class of every primitive the worlds' bodies can refer to,
+// from the ObjectManager as it is now (like the sphere flag above: build the launch graph
+// after the ObjectManager is final).  Without a large primitive the table stays unset and
+// the step is captured exactly as without the knob.
+static void physicsClassifyPrims(Executor *ex)
+{
+    PhysicsHost *ph = ex->physics;
+    PhysicsState &P = ph->hPhys;
+    ph->largeHulls = false;
+    ph->largeError.clear();
+    if (P.maxHullSize <= kMinHullSizeCap) return;
+    auto fail = [&](const char *what) {
+        cudaGetLastError();
+        ph->largeError = what;
+    };
+    i32 info[3] = { 0, 0, 0 };
+    cudaMemset(ph->classInfo, 0, sizeof(info));
+    physPrimExtentKernel<<<ex->numSMs * 4, 256>>>(ex->dState, ph->classInfo);
+    if (cudaMemcpy(info, ph->classInfo, sizeof(info), cudaMemcpyDeviceToHost) != cudaSuccess) {
+        return fail("classifying the collision primitives failed");
+    }
+    if (info[1] != 0) {
+        return fail("MADRONA_B200_MAX_HULL_SIZE needs one ObjectManager shared by all worlds");
+    }
+    const i32 num_prims = info[0];
+    if (num_prims > ph->primClassCapacity) {
+        void *table = nullptr;
+        if (cudaMalloc(&table, (size_t)num_prims) != cudaSuccess) return fail("primitive class table allocation failed");
+        ex->allocations.push_back(table);
+        ph->primClass = (unsigned char *)table;
+        ph->primClassCapacity = num_prims;
+    }
+    if (num_prims > 0) {
+        physClassifyPrimsKernel<<<(num_prims + 255) / 256, 256>>>(ex->dState, ph->primClass, num_prims, ph->classInfo);
+        if (cudaMemcpy(info, ph->classInfo, sizeof(info), cudaMemcpyDeviceToHost) != cudaSuccess) {
+            return fail("classifying the collision primitives failed");
+        }
+    }
+    ph->largeHulls = info[2] != 0;
+    P.primClass = ph->largeHulls ? ph->primClass : nullptr;
+    P.numPrimClasses = ph->largeHulls ? num_prims : 0;
+    cudaMemcpy(&ph->dPhys->primClass, &P.primClass, sizeof(P.primClass), cudaMemcpyHostToDevice);
+    cudaMemcpy(&ph->dPhys->numPrimClasses, &P.numPrimClasses, sizeof(P.numPrimClasses), cudaMemcpyHostToDevice);
+    if (!ph->largeHulls) return;
+    int per_sm = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, physNarrowphaseLargeKernel, kLargeThreads,
+                                                      largeStageBytes(P.maxHullSize)) != cudaSuccess) {
+        cudaGetLastError();
+        per_sm = 0;
+    }
+    ph->largeBlocks = (unsigned)ex->numSMs * (unsigned)per_sm;
 }
 
 void physicsBeforeGraphCapture(Executor *ex)
@@ -2637,6 +2992,7 @@ void physicsBeforeGraphCapture(Executor *ex)
         : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, physNarrowphaseKernel<false>, kNarrowThreads, 0);
     if (e != cudaSuccess) cudaGetLastError();
     ph->narrowBlocks = e == cudaSuccess ? (unsigned)ex->numSMs * (unsigned)per_sm : 0u;
+    physicsClassifyPrims(ex);
 }
 
 void physicsHostDestroy(Executor *ex)
@@ -2664,6 +3020,10 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
         *err = "physics task recorded but PhysicsSystem::registerTypes was never called";
         return false;
     }
+    if (!ph->largeError.empty()) {
+        *err = ph->largeError;
+        return false;
+    }
     EngineState *d = ex->dState;
     const unsigned W = ex->hState->numWorlds;
     const unsigned wgrid = (W + kPhysWarps - 1) / kPhysWarps;
@@ -2688,6 +3048,8 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
             if (rec.userTag != 1) launchSortArchetype(ex, ph->hPhys.jointArchetype, 1, s);
             // the search appends the step's pairs to two empty lists
             cudaMemsetAsync(ph->hPhys.pairCounts, 0, 2 * sizeof(i32), s);
+            // and the pairs with a hull past the staging caps to a third
+            if (ph->largeHulls) cudaMemsetAsync(ph->hPhys.largeCounts, 0, sizeof(i32), s);
             physFindCandidatesKernel<<<wgrid, wblock, 0, s>>>(d);
             break;
         case NodePhysSubstepBegin:
@@ -2700,6 +3062,14 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
             }
             if (ph->spheres) physNarrowphaseKernel<true><<<ph->narrowBlocks, kNarrowThreads, 0, s>>>(d);
             else physNarrowphaseKernel<false><<<ph->narrowBlocks, kNarrowThreads, 0, s>>>(d);
+            if (ph->largeHulls) {
+                if (ph->largeBlocks == 0) {
+                    *err = "large-hull narrowphase occupancy query failed";
+                    return false;
+                }
+                physNarrowphaseLargeKernel<<<ph->largeBlocks, kLargeThreads,
+                                             largeStageBytes(ph->hPhys.maxHullSize), s>>>(d);
+            }
             break;
         case NodePhysSolvePositions:
             physSolvePositionsKernel<<<sgrid, wblock, 0, s>>>(d);

@@ -6,6 +6,8 @@
 
 namespace mb2 {
 
+// MADRONA_B200_MAX_HULL_SIZE (16 when unset), or false and why its value is invalid
+bool physicsMaxHullSize(int *size, std::string *err);
 bool physicsHostCreate(Executor *ex, std::string *err);
 bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *rc, std::string *err);
 void physicsHostDestroy(Executor *ex);

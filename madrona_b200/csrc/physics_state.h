@@ -137,9 +137,20 @@ enum PhysCol : int {
 };
 
 constexpr int kMaxBodyArchetypes = 16;
-constexpr int kMaxHullVerts = 16;     // narrowphase per-thread staging caps
+constexpr int kMaxHullVerts = 16;     // narrowphase staging caps of the group-per-pair path
 constexpr int kMaxHullFaces = 16;
 constexpr int kMaxFaceVerts = 8;
+// MADRONA_B200_MAX_HULL_SIZE: vertices / faces of a hull the warp-per-pair path stages (the
+// reference's narrowphase stages hull - hull pairs in 256-entry halves of its 512-entry arrays)
+constexpr int kMinHullSizeCap = kMaxHullVerts;
+constexpr int kMaxHullSizeCap = 255;
+
+// PhysicsState::primClass: which narrowphase path a collision primitive takes
+enum PrimClass : unsigned char {
+    PrimSmall = 0,      // sphere, plane, or a hull within the three staging caps above
+    PrimLarge = 1,      // a hull within PhysicsState::maxHullSize vertices and faces
+    PrimTooLarge = 2,   // a hull past it: the pair raises ErrPhysicsOverflow
+};
 constexpr int kMaxLevelBodies = 128;  // bodies per world tracked by the contact level scan
 
 struct BodyArchetype {
@@ -189,6 +200,19 @@ struct PhysicsState {
     // [0] hull - hull, [1] other; [2], [3] the narrowphase's item ticket and
     // finished-warp count, zero between launches
     i32 *pairCounts;
+
+    // ---- hulls past the staging caps (MADRONA_B200_MAX_HULL_SIZE > 16)
+    i32 maxHullSize;             // 16: none of the fields below is used
+    // One PrimClass per primitive of the worlds' ObjectManager, written before the launch
+    // graph is captured; null when no primitive is large (the step then runs exactly the
+    // kernels it runs without the knob).  A primitive index past the table (an object
+    // first used after the capture) counts as too large.
+    const unsigned char *primClass;
+    i32 numPrimClasses;
+    // the step's pairs with a large or too large primitive, of every pair type: the third
+    // work list, read by physNarrowphaseLargeKernel
+    PairEntry *largePairs;       // [numWorlds * maxCandidatesPerWorld]
+    i32 *largeCounts;            // [0] pairs, [1] ticket, [2] finished warps (as pairCounts[2], [3])
 };
 
 }

@@ -111,7 +111,12 @@ def _hullpile_objects():
     return hullpile_objects()
 
 
-def _hullpile_desc(name, bodies, compile_flags=()):
+def _hullpile_big_objects():
+    from .objects import hullpile_big_objects
+    return hullpile_big_objects()
+
+
+def _hullpile_desc(name, bodies, compile_flags=(), objects=_hullpile_objects):
     return SimDesc(
         name=name,
         sources=[os.path.join(_ROOT, "hullpile", "sim.cpp")],
@@ -126,7 +131,7 @@ def _hullpile_desc(name, bodies, compile_flags=()):
         pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
         oracle_extra=lambda cfg: [int(cfg.get("seed", 0))],
         defaults={"seed": 0, "layout": 0},
-        objects=_hullpile_objects,
+        objects=objects,
         compile_flags=list(compile_flags),
     )
 
@@ -313,6 +318,12 @@ SIMS: Dict[str, SimDesc] = {
     "hullpile": _hullpile_desc("hullpile", 20),
     # build variant with 60 bodies per world (hull contacts past the 48 staged bodies)
     "hullpile_many": _hullpile_desc("hullpile_many", 60, ["-DHULLPILE_MANY=1"]),
+    # the same two simulators with hulls past those caps (sims/objects.py hullpile_big_specs:
+    # 24-gon prisms, a 16-gon bipyramid, an icosphere, an 11-gon pyramid); on the GPU they
+    # need MADRONA_B200_MAX_HULL_SIZE (tests/test_large_hulls.py)
+    "hullpile_big": _hullpile_desc("hullpile_big", 20, objects=_hullpile_big_objects),
+    "hullpile_big_many": _hullpile_desc("hullpile_big_many", 60, ["-DHULLPILE_MANY=1"],
+                                        objects=_hullpile_big_objects),
     # GPU only: batch ray caster with a real TLAS / BLAS, materials, lights (tests/test_render_bvh.py)
     "gallery": SimDesc(
         name="gallery",

@@ -449,6 +449,75 @@ def hullpile_specs(big_face: bool = False):
     return specs
 
 
+def icosphere_half_edge_mesh(subdiv: int = 1):
+    """An icosahedron with every triangle split in four `subdiv` times and the new vertices
+    pushed out to the circumsphere of radius 0.5 (subdiv = 1: 42 vertices, 80 triangles, 120
+    edges -- a hull past the 16-vertex / 16-face staging caps of the narrowphase)."""
+    g = (1.0 + np.sqrt(5.0)) / 2.0
+    v = [(-1, g, 0), (1, g, 0), (-1, -g, 0), (1, -g, 0), (0, -1, g), (0, 1, g), (0, -1, -g), (0, 1, -g),
+         (g, 0, -1), (g, 0, 1), (-g, 0, -1), (-g, 0, 1)]
+    v = [np.asarray(p, dtype=np.float64) / np.linalg.norm(p) for p in v]
+    faces = [(0, 11, 5), (0, 5, 1), (0, 1, 7), (0, 7, 10), (0, 10, 11), (1, 5, 9), (5, 11, 4), (11, 10, 2),
+             (10, 7, 6), (7, 1, 8), (3, 9, 4), (3, 4, 2), (3, 2, 6), (3, 6, 8), (3, 8, 9), (4, 9, 5),
+             (2, 4, 11), (6, 2, 10), (8, 6, 7), (9, 8, 1)]
+    for _ in range(subdiv):
+        mid = {}
+
+        def midpoint(i, j):
+            key = (min(i, j), max(i, j))
+            if key not in mid:
+                m = v[i] + v[j]
+                v.append(m / np.linalg.norm(m))
+                mid[key] = len(v) - 1
+            return mid[key]
+
+        split = []
+        for a, b, c in faces:
+            ab, bc, ca = midpoint(a, b), midpoint(b, c), midpoint(c, a)
+            split += [(a, ab, ca), (b, bc, ab), (c, ca, bc), (ab, bc, ca)]
+        faces = split
+    verts = (0.5 * np.asarray(v)).astype(np.float32)
+    return build_half_edge_mesh(verts, orient_faces(verts, faces))
+
+
+def hullpile_big_specs():
+    """hullpile_specs() with hulls past the narrowphase's staging caps (16 vertices, 16 faces,
+    8-vertex faces) in place of five of its objects, same SimObject order: OctPrism and
+    Pedestal are 24-gon prisms (48 vertices, 26 faces, two 24-vertex faces), Bipyramid a
+    16-gon bipyramid (18 vertices, 32 faces), Tetra an icosphere (42 vertices, 80 faces),
+    PentaPyramid an 11-gon pyramid with an off-centre apex (12 vertices and 12 faces: large
+    only through its 11-vertex base).  Box, Wedge, Ball, Dumbbell, CappedBox, Plane and Wall
+    stay, so a pile has large - large, large - small, large - plane, sphere - large and
+    small - small pairs in one world."""
+    specs = hullpile_specs()
+    prism = ngon_prism_half_edge_mesh(24)
+    for obj, mesh in ((2, prism), (3, bipyramid_half_edge_mesh(16)), (4, icosphere_half_edge_mesh(1)),
+                      (5, pyramid_half_edge_mesh(11, (0.15, 0.1))), (11, prism)):
+        specs[obj] = dict(prims=[mesh], meta=specs[obj]["meta"])
+    return specs
+
+
+def hullpile_big_objects() -> Tuple[bytes, List[int]]:
+    return build_compound_objects(hullpile_big_specs())
+
+
+def hull_size_class(mesh, max_hull_size: int = 16) -> str:
+    """"small" (within the staging caps of the group-per-pair narrowphase: 16 vertices, 16
+    faces, 8 vertices per face), "large" (within max_hull_size vertices and faces) or
+    "too large": what the engine's primitive class table holds for a hull."""
+    he = mesh["half_edges"]
+    longest = 0
+    for base in mesh["face_base"]:
+        h, n = int(he[int(base)][0]), 1
+        while h != int(base) and n < len(he):
+            h, n = int(he[h][0]), n + 1
+        longest = max(longest, n)
+    nv, nf = len(mesh["vertices"]), len(mesh["planes"])
+    if nv > max_hull_size or nf > max_hull_size or longest > max_hull_size:
+        return "too large"
+    return "large" if nv > 16 or nf > 16 or longest > 8 else "small"
+
+
 def triggers_objects() -> Tuple[bytes, List[int]]:
     """Objects of sims/triggers, in SimObject order: Agent, Pickup, Wall, Floor (plane),
     Dumbbell (two unit boxes side by side along x, centred 0.6 from the origin: a compound
