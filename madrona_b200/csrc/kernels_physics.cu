@@ -537,6 +537,19 @@ struct CandidateScratch {
     StagedLeaf leaves[kPhysWarps][kMaxStagedLeaves];
 };
 
+// Appends candidate i of world w to `list` on the lanes where `take` is set: one atomic
+// per warp, the lanes' entries in lane order.
+__device__ __forceinline__ void appendPairs(const PairList &list, const bool take, const i32 w, const i32 i,
+                                            const int lane)
+{
+    const unsigned mask = __ballot_sync(0xffffffffu, take);
+    if (!mask) return;
+    i32 at = 0;
+    if (lane == 0) at = atomicAdd(&list.counters->count, __popc(mask));
+    at = __shfl_sync(0xffffffffu, at, 0);
+    if (take) list.entries[at + __popc(mask & ((1u << lane) - 1u))] = PairEntry { w, i };
+}
+
 // Candidate pairs of one world, in the CPU backend's order (bodies: archetype
 // ascending, then row; partners of a body: BVH report order).  The set a
 // traversal reports for body a is { leaf b : slotBox(b) overlaps leafBox(a) }
@@ -675,7 +688,7 @@ __device__ void phaseFindCandidates(EngineState &S, const PhysicsState &P, const
                             const u32 a_rel = c / sl.prims, b_rel = c % sl.prims;
                             const u32 a_prim = self_base + a_rel, b_prim = sl.primBase + b_rel;
                             const u32 ta = objs.prims[a_prim].type, tb = objs.prims[b_prim].type;
-                            const u32 cls = (ta | tb) << 16;
+                            const u32 cls = (ta | tb) << 16;      // the PairClass
                             const u32 rel = a_rel | (b_rel << 8) | (ta > tb ? 1u << 16 : 0u);
                             out[at] = ta > tb
                                 ? Candidate { b_prim, a_prim, sl.row, row, sl.arch | (b.archetype << 8) | cls,
@@ -712,26 +725,12 @@ __device__ void phaseFindCandidates(EngineState &S, const PhysicsState &P, const
                 large = (pa < n ? prim_class[pa] : (u32)PrimTooLarge) != PrimSmall ||
                         (pb < n ? prim_class[pb] : (u32)PrimTooLarge) != PrimSmall;
             }
-            const unsigned large_mask = __ballot_sync(0xffffffffu, large);
-            if (large_mask) {
-                i32 large_at = 0;
-                if (lane == 0) large_at = atomicAdd(&P.largeCounts[0], __popc(large_mask));
-                large_at = __shfl_sync(0xffffffffu, large_at, 0);
-                if (large) P.largePairs[large_at + __popc(large_mask & ((1u << lane) - 1u))] = PairEntry { w, i };
-                valid = valid && !large;
-            }
+            appendPairs(P.largePairs, large, w, i, lane);
+            valid = valid && !large;
         }
-        const bool hh = valid && (out[i].arch >> 16) == 2u;
-        const unsigned hh_mask = __ballot_sync(0xffffffffu, hh);
-        const unsigned other_mask = __ballot_sync(0xffffffffu, valid && !hh);
-        i32 hh_at = 0, other_at = 0;
-        if (lane == 0 && hh_mask) hh_at = atomicAdd(&P.pairCounts[0], __popc(hh_mask));
-        if (lane == 0 && other_mask) other_at = atomicAdd(&P.pairCounts[1], __popc(other_mask));
-        hh_at = __shfl_sync(0xffffffffu, hh_at, 0);
-        other_at = __shfl_sync(0xffffffffu, other_at, 0);
-        const unsigned below = (1u << lane) - 1u;
-        if (hh) P.hullPairs[hh_at + __popc(hh_mask & below)] = PairEntry { w, i };
-        else if (valid) P.otherPairs[other_at + __popc(other_mask & below)] = PairEntry { w, i };
+        const bool hh = valid && (out[i].arch >> 16) == PairHullHull;
+        appendPairs(P.hullPairs, hh, w, i, lane);
+        appendPairs(P.otherPairs, valid && !hh, w, i, lane);
     }
 }
 
@@ -1019,121 +1018,6 @@ __device__ __forceinline__ PairSetup setupPair(const ObjectManager &objs, const 
     return ps;
 }
 
-// sphere (a) - hull (b): GJK closest point of the hull to the sphere centre, SAT
-// over the face planes when the centre is inside (narrowphase.cpp:1326-1402).
-// Out of line and by value: rare in the box-world fixtures, and inlining the GJK
-// loop doubles the narrowphase kernel's code size.
-struct SphereHullResult {
-    Vector3 point;
-    Vector3 normal;
-    float depth;
-    i32 hit;          // 1 contact, 0 none, -1 hull too large for the staging array
-};
-
-__device__ __noinline__ SphereHullResult sphereHullContact(Vector3 a_pos, float radius, Vector3 b_pos,
-                                                           Quat b_rot, Diag3x3 b_scale,
-                                                           const HalfEdgeMesh *mesh)
-{
-    const HalfEdgeMesh &bm = *mesh;
-    SphereHullResult res { Vector3::zero(), Vector3::zero(), 0.f, 0 };
-    if (bm.numVertices > (u32)kMaxHullVerts) {
-        res.hit = -1;
-        return res;
-    }
-    // the hull relative to the sphere centre, so the query point is the origin
-    const Vector3 hull_origin = b_pos - a_pos;
-    const Mat3x3 rot = Mat3x3::fromQuat(b_rot);
-    const Mat3x3 vert_m = rot * b_scale;
-    const Mat3x3 norm_m = rot * b_scale.inv();
-    Vector3 verts[kMaxHullVerts];
-#pragma unroll 1
-    for (u32 i = 0; i < bm.numVertices; i++) verts[i] = vert_m * bm.vertices[i] + hull_origin;
-
-    Vector3 to_hull;
-    const float dist2 = madrona::geo::hullVerticesClosestPointToOriginGJK(verts, bm.numVertices, 1e-10f,
-                                                                         &to_hull);
-    if (dist2 > radius * radius) return res;
-
-    if (dist2 == 0.f) {
-        // centre inside the hull: least-penetrated face (SAT over the face planes)
-        float max_sep = -FLT_MAX;
-        Vector3 sep_normal = Vector3::zero();
-#pragma unroll 1
-        for (u32 f = 0; f < bm.numFaces; f++) {
-            const Plane local = bm.facePlanes[f];
-            const Vector3 on_plane = vert_m * (local.normal * local.d) + hull_origin;
-            const Vector3 n = (norm_m * local.normal).normalize();
-            const float face_dist = -dot(n, on_plane);
-            if (face_dist > max_sep) {
-                max_sep = face_dist;
-                sep_normal = n;
-            }
-        }
-        if (max_sep > 0.f) return res;      // GJK and SAT disagree by rounding
-        res.point = a_pos + sep_normal * radius;
-        res.normal = sep_normal;
-        res.depth = -max_sep;
-    } else {
-        const float to_hull_len = sqrtf(dist2);
-        const Vector3 normal = to_hull / to_hull_len;
-        res.point = a_pos + normal * radius;
-        res.normal = -normal;
-        res.depth = radius - to_hull_len;
-    }
-    res.hit = 1;
-    return res;
-}
-
-// sphere-sphere (1), sphere-plane (5), sphere-hull (3): one lane of the group.
-// Single-point contacts store (ref, alt) = (b, a).
-template <bool SPHERE_HULL>
-__device__ bool singlePointPair(EngineState &S, const PairSetup &ps, Contact &out)
-{
-    switch (ps.test) {
-    case 1: {
-        const float ra = ps.aScale.d0 * ps.aPrim->sphereRadius;
-        const float rb = ps.bScale.d0 * ps.bPrim->sphereRadius;
-        const Vector3 to_b = ps.bPos - ps.aPos;
-        const float dist = to_b.length();
-        if (dist > ra + rb) return false;
-        const Vector3 n = dist > 0.f ? to_b / dist : madrona::math::up;
-        writeSinglePointContact(out, ps.bArch, ps.bRow, ps.bInfo, ps.aArch, ps.aRow, ps.aInfo,
-                                ps.aPos + ra * n, n, ra + rb - dist);
-        return true;
-    }
-    case 5: {
-        const float ra = ps.aScale.d0 * ps.aPrim->sphereRadius;
-        const Vector3 n = ps.bRot.rotateVec(Vector3 { 0, 0, 1 });
-        const float d = n.dot(ps.bPos);
-        const float t = n.dot(ps.aPos) - d;
-        const float pen = ra - t;
-        if (pen < 0) return false;
-        writeSinglePointContact(out, ps.bArch, ps.bRow, ps.bInfo, ps.aArch, ps.aRow, ps.aInfo,
-                                ps.aPos - t * n, n, pen);
-        return true;
-    }
-    case 3: {
-        if constexpr (SPHERE_HULL) {
-            const SphereHullResult r = sphereHullContact(ps.aPos, ps.aScale.d0 * ps.aPrim->sphereRadius,
-                                                         ps.bPos, ps.bRot, ps.bScale, &ps.bPrim->hull);
-            if (r.hit < 0) atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
-            if (r.hit <= 0) return false;
-            writeSinglePointContact(out, ps.bArch, ps.bRow, ps.bInfo, ps.aArch, ps.aRow, ps.aInfo,
-                                    r.point, r.normal, r.depth);
-            return true;
-        } else {
-            // a sphere appeared after the launch graph was built without the
-            // sphere-hull path: rebuild the launch graph
-            atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
-            return false;
-        }
-    }
-    default:
-        atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
-        return false;
-    }
-}
-
 struct HullScratch {
     Vector3 verts[2 * kMaxHullVerts];
     Plane planes[2 * kMaxHullFaces];
@@ -1358,6 +1242,148 @@ __device__ int groupManifold(unsigned gm, int sub, const Plane &ref_plane, const
         writeContactPoint(out, k, kept[src], depths[src]);
     }
     return 4;
+}
+
+struct SphereHullResult {
+    Vector3 point;
+    Vector3 normal;
+    float depth;
+    i32 hit;          // 1 contact, 0 none, -1 hull too large for the staging array
+};
+
+// sphere (a) - hull (b) by the G lanes of a group: GJK closest point of the hull to the
+// sphere centre on the group's first lane, SAT over the face planes when the centre is
+// inside, the faces dealt to the lanes (narrowphase.cpp:1326-1402).  The lanes stage the
+// placed vertices in `verts`, which the caller checked the hull against.  `hit` is the
+// same on every lane; point, normal and depth are set on the group's first lane.
+template <int G>
+__device__ __forceinline__ SphereHullResult sphereHullGroup(Vector3 a_pos, float radius, Vector3 b_pos, Quat b_rot,
+                                                            Diag3x3 b_scale, const HalfEdgeMesh &bm, Vector3 *verts,
+                                                            const unsigned gm, const int sub)
+{
+    SphereHullResult res { Vector3::zero(), Vector3::zero(), 0.f, 0 };
+    // the hull relative to the sphere centre, so the query point is the origin
+    const Vector3 hull_origin = b_pos - a_pos;
+    const Mat3x3 rot = Mat3x3::fromQuat(b_rot);
+    const Mat3x3 vert_m = rot * b_scale;
+    const Mat3x3 norm_m = rot * b_scale.inv();
+#pragma unroll 1
+    for (u32 i = (u32)sub; i < bm.numVertices; i += G) verts[i] = vert_m * bm.vertices[i] + hull_origin;
+    if constexpr (G > 1) __syncwarp(gm);
+
+    Vector3 to_hull = Vector3::zero();
+    float dist2 = 0.f;
+    if (sub == 0) dist2 = madrona::geo::hullVerticesClosestPointToOriginGJK(verts, bm.numVertices, 1e-10f, &to_hull);
+    if constexpr (G > 1) dist2 = __shfl_sync(gm, dist2, __ffs(gm) - 1);
+    if (dist2 > radius * radius) return res;
+
+    if (dist2 == 0.f) {
+        // centre inside the hull: least-penetrated face, the first maximum of the face scan
+        float best = -FLT_MAX;
+        i32 best_face = 0;
+        Vector3 best_n = Vector3::zero();
+        bool have = false;
+#pragma unroll 1
+        for (u32 f = (u32)sub; f < bm.numFaces; f += G) {
+            const Plane local = bm.facePlanes[f];
+            const Vector3 on_plane = vert_m * (local.normal * local.d) + hull_origin;
+            const Vector3 n = (norm_m * local.normal).normalize();
+            const float face_dist = -dot(n, on_plane);
+            if (face_dist > best) {
+                best = face_dist;
+                best_face = (i32)f;
+                best_n = n;
+                have = true;
+            }
+        }
+        const Winner win = groupFirstBest<false, G>(gm, best, best_face, have);
+        // no face beat the scan's start value: it keeps -FLT_MAX and a zero normal
+        const bool found = win.idx != 0x7fffffff;
+        const float max_sep = found ? win.sep : -FLT_MAX;
+        if (max_sep > 0.f) return res;      // GJK and SAT disagree by rounding
+        Vector3 sep_normal = best_n;
+        if constexpr (G > 1) {
+            // the winning lane's normal to the group's first lane
+            const unsigned owner = __ballot_sync(gm, have && best_face == win.idx);
+            const int src = owner ? __ffs(owner) - 1 : __ffs(gm) - 1;
+            sep_normal.x = __shfl_sync(gm, best_n.x, src);
+            sep_normal.y = __shfl_sync(gm, best_n.y, src);
+            sep_normal.z = __shfl_sync(gm, best_n.z, src);
+        }
+        res.point = a_pos + sep_normal * radius;
+        res.normal = sep_normal;
+        res.depth = -max_sep;
+    } else {
+        const float to_hull_len = sqrtf(dist2);
+        const Vector3 normal = to_hull / to_hull_len;
+        res.point = a_pos + normal * radius;
+        res.normal = -normal;
+        res.depth = radius - to_hull_len;
+    }
+    res.hit = 1;
+    return res;
+}
+
+// One lane of physNarrowphaseKernel, the vertices in a per-thread array.  Out of line and
+// by value: rare in the box-world fixtures, and inlining the GJK loop doubles the
+// narrowphase kernel's code size.
+__device__ __noinline__ SphereHullResult sphereHullContact(Vector3 a_pos, float radius, Vector3 b_pos,
+                                                           Quat b_rot, Diag3x3 b_scale,
+                                                           const HalfEdgeMesh *mesh)
+{
+    if (mesh->numVertices > (u32)kMaxHullVerts) return SphereHullResult { Vector3::zero(), Vector3::zero(), 0.f, -1 };
+    Vector3 verts[kMaxHullVerts];
+    return sphereHullGroup<1>(a_pos, radius, b_pos, b_rot, b_scale, *mesh, verts, 1u << (threadIdx.x & 31), 0);
+}
+
+// sphere - sphere, sphere - plane, sphere - hull: one lane of the group.
+// Single-point contacts store (ref, alt) = (b, a).
+template <bool SPHERE_HULL>
+__device__ bool singlePointPair(EngineState &S, const PairSetup &ps, Contact &out)
+{
+    switch (ps.test) {
+    case PairSphereSphere: {
+        const float ra = ps.aScale.d0 * ps.aPrim->sphereRadius;
+        const float rb = ps.bScale.d0 * ps.bPrim->sphereRadius;
+        const Vector3 to_b = ps.bPos - ps.aPos;
+        const float dist = to_b.length();
+        if (dist > ra + rb) return false;
+        const Vector3 n = dist > 0.f ? to_b / dist : madrona::math::up;
+        writeSinglePointContact(out, ps.bArch, ps.bRow, ps.bInfo, ps.aArch, ps.aRow, ps.aInfo,
+                                ps.aPos + ra * n, n, ra + rb - dist);
+        return true;
+    }
+    case PairSpherePlane: {
+        const float ra = ps.aScale.d0 * ps.aPrim->sphereRadius;
+        const Vector3 n = ps.bRot.rotateVec(Vector3 { 0, 0, 1 });
+        const float d = n.dot(ps.bPos);
+        const float t = n.dot(ps.aPos) - d;
+        const float pen = ra - t;
+        if (pen < 0) return false;
+        writeSinglePointContact(out, ps.bArch, ps.bRow, ps.bInfo, ps.aArch, ps.aRow, ps.aInfo,
+                                ps.aPos - t * n, n, pen);
+        return true;
+    }
+    case PairSphereHull: {
+        if constexpr (SPHERE_HULL) {
+            const SphereHullResult r = sphereHullContact(ps.aPos, ps.aScale.d0 * ps.aPrim->sphereRadius,
+                                                         ps.bPos, ps.bRot, ps.bScale, &ps.bPrim->hull);
+            if (r.hit < 0) atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
+            if (r.hit <= 0) return false;
+            writeSinglePointContact(out, ps.bArch, ps.bRow, ps.bInfo, ps.aArch, ps.aRow, ps.aInfo,
+                                    r.point, r.normal, r.depth);
+            return true;
+        } else {
+            // a sphere appeared after the launch graph was built without the
+            // sphere-hull path: rebuild the launch graph
+            atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
+            return false;
+        }
+    }
+    default:
+        atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
+        return false;
+    }
 }
 
 // hull (a) - plane (b, the reference).  The hull is never stored: each lane places
@@ -1660,9 +1686,9 @@ __device__ bool hullHullGroup(EngineState &S, const PairSetup &ps, const HullSta
 // by the candidate search).  The unit of work is a warp item: kGroupLanes-lane
 // groups on 4 hull - hull pairs, or kPlaneLanes-lane groups on 8 other pairs.
 // Items are numbered [hull - hull items][other items], so the long chains start
-// first, and handed out in that order by a ticket (one atomic per warp and item,
-// fetched while the previous item runs): both classes share every SM, neither
-// waits for a wave of the other, and a warp that drew short pairs takes more.
+// first, and handed out in that order by hullPairs' ticket (forEachTicket): both
+// classes share every SM, neither waits for a wave of the other, and a warp that
+// drew short pairs takes more.
 // Each pair writes only its own contact slot and candHit entry, so which warp
 // takes which pair changes no result.  orderContacts (prologue of the position
 // solve) lists each world's hits in candidate order and assigns the dependency
@@ -1686,6 +1712,32 @@ constexpr int kPlaneLanes = 4;
 constexpr int kHullPairsPerWarp = 32 / kGroupLanes;
 constexpr int kPlanePairsPerWarp = 32 / kPlaneLanes;
 
+// Hands the work items [0, items) out to the warps of a persistent grid (`warps` per
+// block) by the ticket in `c`: one atomic per warp and item, fetched while the previous
+// item runs.  The warp runs run(item) on all its lanes and syncs before its next item,
+// which may reuse its staging.  Every warp has taken its last ticket before it counts
+// itself out, so the last one out can zero the ticket and the finished count for the next
+// launch.
+template <typename Run>
+__device__ __forceinline__ void forEachTicket(PairListCounters *c, const i32 items, const int warps,
+                                              const int lane, Run &&run)
+{
+    i32 item = 0;
+    if (lane == 0) item = atomicAdd(&c->ticket, 1);
+    item = __shfl_sync(0xffffffffu, item, 0);
+    while (item < items) {
+        i32 next = 0;
+        if (lane == 0) next = atomicAdd(&c->ticket, 1);    // in flight while this item runs
+        run(item);
+        __syncwarp();
+        item = __shfl_sync(0xffffffffu, next, 0);
+    }
+    if (lane == 0 && atomicAdd(&c->finished, 1) == (i32)gridDim.x * warps - 1) {
+        c->ticket = 0;
+        c->finished = 0;
+    }
+}
+
 template <bool SPHERE_HULL>
 __global__ void __launch_bounds__(kNarrowThreads, SPHERE_HULL ? kNarrowMinBlocksSpheres : kNarrowMinBlocks)
 physNarrowphaseKernel(EngineState *Sp)
@@ -1700,63 +1752,37 @@ physNarrowphaseKernel(EngineState *Sp)
     } scratch[kNarrowWarps];
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x / 32;
-    const i32 num_hull = P.pairCounts[0], num_other = P.pairCounts[1];
+    const i32 num_hull = P.hullPairs.counters->count, num_other = P.otherPairs.counters->count;
     const i32 hull_items = (num_hull + kHullPairsPerWarp - 1) / kHullPairsPerWarp;
     const i32 items = hull_items + (num_other + kPlanePairsPerWarp - 1) / kPlanePairsPerWarp;
-    i32 *const ticket = &P.pairCounts[2];
-    i32 item = 0;
-    if (lane == 0) item = atomicAdd(ticket, 1);
-    item = __shfl_sync(0xffffffffu, item, 0);
-
-    while (item < hull_items) {
-        i32 next = 0;
-        if (lane == 0) next = atomicAdd(ticket, 1);    // in flight while this item runs
-        const int sub = lane % kGroupLanes;
-        const int group = lane / kGroupLanes;
-        const unsigned gm = ((1u << kGroupLanes) - 1u) << (group * kGroupLanes);
-        const i32 e = item * kHullPairsPerWarp + group;
-        if (e < num_hull) {
-            const PairEntry ent = P.hullPairs[e];
-            const size_t slot = (size_t)ent.world * P.maxCandidatesPerWorld + ent.cand;
-            const PairSetup ps = setupPair(worldObjects(S, P, ent.world), P.candidates[slot]);
-            const bool made = ps.test != 0 && hullHullGroup<kGroupLanes>(
-                S, ps, smallHullStage(scratch[warp].hull[group]), gm, sub, P.contacts[slot]);
-            if (sub == 0) P.candHit[slot] = made ? 1 : 0;
-        }
-        // the warp's next item may use its scratch in the other layout
-        __syncwarp();
-        item = __shfl_sync(0xffffffffu, next, 0);
-    }
-    while (item < items) {
-        i32 next = 0;
-        if (lane == 0) next = atomicAdd(ticket, 1);
-        const int sub = lane % kPlaneLanes;
-        const int group = lane / kPlaneLanes;
-        const unsigned gm = ((1u << kPlaneLanes) - 1u) << (group * kPlaneLanes);
-        const i32 e = (item - hull_items) * kPlanePairsPerWarp + group;
-        if (e < num_other) {
-            const PairEntry ent = P.otherPairs[e];
-            const size_t slot = (size_t)ent.world * P.maxCandidatesPerWorld + ent.cand;
-            const PairSetup ps = setupPair(worldObjects(S, P, ent.world), P.candidates[slot]);
-            bool made = false;
-            if (ps.test == 6) {
+    // Both kinds of item share one copy of the pair's setup: with a copy per kind the
+    // kernel needs more registers than its launch bounds allow and spills.
+    forEachTicket(P.hullPairs.counters, items, kNarrowWarps, lane, [&](const i32 item) {
+        const bool hull = item < hull_items;
+        const int sub = hull ? lane % kGroupLanes : lane % kPlaneLanes;
+        const int group = hull ? lane / kGroupLanes : lane / kPlaneLanes;
+        const unsigned gm = hull ? ((1u << kGroupLanes) - 1u) << (group * kGroupLanes)
+                                 : ((1u << kPlaneLanes) - 1u) << (group * kPlaneLanes);
+        const i32 e = hull ? item * kHullPairsPerWarp + group : (item - hull_items) * kPlanePairsPerWarp + group;
+        if (e >= (hull ? num_hull : num_other)) return;
+        const PairEntry ent = (hull ? P.hullPairs : P.otherPairs).entries[e];
+        const size_t slot = (size_t)ent.world * P.maxCandidatesPerWorld + ent.cand;
+        const PairSetup ps = setupPair(worldObjects(S, P, ent.world), P.candidates[slot]);
+        bool made = false;
+        if (ps.test != 0) {
+            if (hull) {
+                made = hullHullGroup<kGroupLanes>(S, ps, smallHullStage(scratch[warp].hull[group]), gm, sub,
+                                                  P.contacts[slot]);
+            } else if (ps.test == PairHullPlane) {
                 made = hullPlaneGroup<kPlaneLanes>(S, ps, scratch[warp].plane[group], gm, sub, P.contacts[slot]);
-            } else if (ps.test != 0) {
+            } else {
                 i32 hit = 0;
                 if (sub == 0) hit = singlePointPair<SPHERE_HULL>(S, ps, P.contacts[slot]) ? 1 : 0;
                 made = __shfl_sync(gm, hit, __ffs(gm) - 1) != 0;
             }
-            if (sub == 0) P.candHit[slot] = made ? 1 : 0;
         }
-        __syncwarp();
-        item = __shfl_sync(0xffffffffu, next, 0);
-    }
-    // Every warp has taken its last ticket before it counts itself out, so the last
-    // one out can zero the ticket for the next launch.
-    if (lane == 0 && atomicAdd(&P.pairCounts[3], 1) == (i32)gridDim.x * kNarrowWarps - 1) {
-        P.pairCounts[2] = 0;
-        P.pairCounts[3] = 0;
-    }
+        if (sub == 0) P.candHit[slot] = made ? 1 : 0;
+    });
 }
 
 // ---- hulls past the staging caps: one warp per pair --------------------------------------
@@ -1785,74 +1811,6 @@ __device__ __forceinline__ HullStage largeHullStage(unsigned char *base, const i
                        n, n, n, 2 * n };
 }
 
-// sphere (a) - hull (b) by one warp, the arithmetic of sphereHullContact: the translated
-// vertices are staged by all lanes, GJK runs on lane 0, the face scan of a centre inside
-// the hull is dealt to the lanes ("first strictly greater" == lowest index among maxima).
-// Lane 0 writes the contact; returns on every lane whether there is one.
-__device__ bool sphereHullWarp(const PairSetup &ps, const HullStage &st, const int lane, Contact &out)
-{
-    const HalfEdgeMesh &bm = ps.bPrim->hull;
-    const float radius = ps.aScale.d0 * ps.aPrim->sphereRadius;
-    const Vector3 a_pos = ps.aPos;
-    const Vector3 hull_origin = ps.bPos - a_pos;
-    const Mat3x3 rot = Mat3x3::fromQuat(ps.bRot);
-    const Mat3x3 vert_m = rot * ps.bScale;
-    const Mat3x3 norm_m = rot * ps.bScale.inv();
-    Vector3 *verts = st.vertsA;     // maxVerts entries: the caller checked the hull against it
-#pragma unroll 1
-    for (u32 i = (u32)lane; i < bm.numVertices; i += 32) verts[i] = vert_m * bm.vertices[i] + hull_origin;
-    __syncwarp();
-
-    Vector3 to_hull = Vector3::zero();
-    float dist2 = 0.f;
-    if (lane == 0) {
-        dist2 = madrona::geo::hullVerticesClosestPointToOriginGJK(verts, bm.numVertices, 1e-10f, &to_hull);
-    }
-    dist2 = __shfl_sync(0xffffffffu, dist2, 0);
-    if (dist2 > radius * radius) return false;
-
-    if (dist2 == 0.f) {
-        float best = -FLT_MAX;
-        i32 best_face = 0;
-        Vector3 best_n = Vector3::zero();
-        bool have = false;
-#pragma unroll 1
-        for (u32 f = (u32)lane; f < bm.numFaces; f += 32) {
-            const Plane local = bm.facePlanes[f];
-            const Vector3 on_plane = vert_m * (local.normal * local.d) + hull_origin;
-            const Vector3 n = (norm_m * local.normal).normalize();
-            const float face_dist = -dot(n, on_plane);
-            if (face_dist > best) {
-                best = face_dist;
-                best_face = (i32)f;
-                best_n = n;
-                have = true;
-            }
-        }
-        const Winner win = groupFirstBest<false, 32>(0xffffffffu, best, best_face, have);
-        // no face beat the scan's start value: it keeps -FLT_MAX and a zero normal
-        const float max_sep = win.idx == 0x7fffffff ? -FLT_MAX : win.sep;
-        if (max_sep > 0.f) return false;      // GJK and SAT disagree by rounding
-        const unsigned owner = __ballot_sync(0xffffffffu, have && best_face == win.idx);
-        if (owner && lane == __ffs(owner) - 1) {
-            writeSinglePointContact(out, ps.bArch, ps.bRow, ps.bInfo, ps.aArch, ps.aRow, ps.aInfo,
-                                    a_pos + best_n * radius, best_n, -max_sep);
-        } else if (!owner && lane == 0) {
-            const Vector3 zero = Vector3::zero();
-            writeSinglePointContact(out, ps.bArch, ps.bRow, ps.bInfo, ps.aArch, ps.aRow, ps.aInfo,
-                                    a_pos + zero * radius, zero, -max_sep);
-        }
-        return true;
-    }
-    if (lane == 0) {
-        const float to_hull_len = sqrtf(dist2);
-        const Vector3 normal = to_hull / to_hull_len;
-        writeSinglePointContact(out, ps.bArch, ps.bRow, ps.bInfo, ps.aArch, ps.aRow, ps.aInfo,
-                                a_pos + normal * radius, -normal, radius - to_hull_len);
-    }
-    return true;
-}
-
 __global__ void __launch_bounds__(kLargeThreads, 1)
 physNarrowphaseLargeKernel(EngineState *Sp)
 {
@@ -1864,46 +1822,37 @@ physNarrowphaseLargeKernel(EngineState *Sp)
     const int warp = threadIdx.x / 32;
     const int cap = P.maxHullSize;
     const HullStage st = largeHullStage(large_stage + (size_t)warp * cap * kLargeStageBytesPerEntry, cap);
-    const i32 num_pairs = P.largeCounts[0];
-    i32 *const ticket = &P.largeCounts[1];
-    i32 item = 0;
-    if (lane == 0) item = atomicAdd(ticket, 1);
-    item = __shfl_sync(0xffffffffu, item, 0);
-
-    while (item < num_pairs) {
-        i32 next = 0;
-        if (lane == 0) next = atomicAdd(ticket, 1);    // in flight while this pair runs
-        const PairEntry ent = P.largePairs[item];
+    forEachTicket(P.largePairs.counters, P.largePairs.counters->count, kLargeWarps, lane, [&](const i32 item) {
+        const PairEntry ent = P.largePairs.entries[item];
         const size_t slot = (size_t)ent.world * P.maxCandidatesPerWorld + ent.cand;
         const PairSetup ps = setupPair(worldObjects(S, P, ent.world), P.candidates[slot]);
         bool made = false;
         if (ps.test != 0) {
             // side a is a hull except in sphere - hull pairs, side b except in hull - plane pairs
-            const HalfEdgeMesh *ha = ps.test != 3 ? &ps.aPrim->hull : nullptr;
-            const HalfEdgeMesh *hb = ps.test != 6 ? &ps.bPrim->hull : nullptr;
+            const HalfEdgeMesh *ha = ps.test != PairSphereHull ? &ps.aPrim->hull : nullptr;
+            const HalfEdgeMesh *hb = ps.test != PairHullPlane ? &ps.bPrim->hull : nullptr;
             const bool fits = (!ha || (ha->numVertices <= (u32)cap && ha->numFaces <= (u32)cap)) &&
                               (!hb || (hb->numVertices <= (u32)cap && hb->numFaces <= (u32)cap));
-            if (!fits || (ps.test != 2 && ps.test != 3 && ps.test != 6)) {
+            if (!fits || (ps.test != PairHullHull && ps.test != PairSphereHull && ps.test != PairHullPlane)) {
                 if (lane == 0) atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
-            } else if (ps.test == 2) {
+            } else if (ps.test == PairHullHull) {
                 made = hullHullGroup<32>(S, ps, st, 0xffffffffu, lane, P.contacts[slot]);
-            } else if (ps.test == 6) {
+            } else if (ps.test == PairHullPlane) {
                 LargePlaneStage plane_stage { st.clipA, st.clipB, st.depths, st.maxFaceVerts };
                 made = hullPlaneGroup<32>(S, ps, plane_stage, 0xffffffffu, lane, P.contacts[slot]);
             } else {
-                made = sphereHullWarp(ps, st, lane, P.contacts[slot]);
+                const SphereHullResult r = sphereHullGroup<32>(ps.aPos, ps.aScale.d0 * ps.aPrim->sphereRadius, ps.bPos,
+                                                               ps.bRot, ps.bScale, ps.bPrim->hull, st.vertsA,
+                                                               0xffffffffu, lane);
+                made = r.hit > 0;
+                if (made && lane == 0) {
+                    writeSinglePointContact(P.contacts[slot], ps.bArch, ps.bRow, ps.bInfo, ps.aArch, ps.aRow,
+                                            ps.aInfo, r.point, r.normal, r.depth);
+                }
             }
         }
         if (lane == 0) P.candHit[slot] = made ? 1 : 0;
-        // the stage is reused by the warp's next pair
-        __syncwarp();
-        item = __shfl_sync(0xffffffffu, next, 0);
-    }
-    // as in physNarrowphaseKernel: the last warp out zeroes the ticket for the next launch
-    if (lane == 0 && atomicAdd(&P.largeCounts[2], 1) == (i32)gridDim.x * kLargeWarps - 1) {
-        P.largeCounts[1] = 0;
-        P.largeCounts[2] = 0;
-    }
+    });
 }
 
 // ---- primitive classes, once before the launch graph is captured --------------------------
@@ -2884,14 +2833,21 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::stri
         cudaMemset(*p, 0, bytes);
         return true;
     };
+    // The step's work lists.  Their counters are one array, hull - hull, other, large, so
+    // one memset before the candidate search resets the lists a step uses.
+    PairListCounters *pair_counters = nullptr;
+    auto alloc_list = [&](PairList &list, int k) {
+        list.counters = pair_counters + k;
+        return alloc((void **)&list.entries, sizeof(PairEntry) * W * P.maxCandidatesPerWorld);
+    };
     if (!alloc((void **)&P.candidates, sizeof(Candidate) * W * P.maxCandidatesPerWorld) ||
         !alloc((void **)&P.candCounts, sizeof(i32) * W) ||
         !alloc((void **)&P.contacts, sizeof(Contact) * W * P.maxCandidatesPerWorld) ||
         !alloc((void **)&P.candHit, sizeof(i32) * W * P.maxCandidatesPerWorld) ||
         !alloc((void **)&P.contactOrder, sizeof(i32) * W * P.maxContactsPerWorld) ||
-        !alloc((void **)&P.hullPairs, sizeof(PairEntry) * W * P.maxCandidatesPerWorld) ||
-        !alloc((void **)&P.otherPairs, sizeof(PairEntry) * W * P.maxCandidatesPerWorld) ||
-        !alloc((void **)&P.pairCounts, sizeof(i32) * 4) ||
+        !alloc((void **)&pair_counters, sizeof(PairListCounters) * 3) ||
+        !alloc_list(P.hullPairs, 0) ||
+        !alloc_list(P.otherPairs, 1) ||
         !alloc((void **)&P.contactCounts, sizeof(i32) * W) ||
         !alloc((void **)&P.contactMaxLevel, sizeof(i32) * W)) {
         *err = "physics buffers allocation failed";
@@ -2902,8 +2858,7 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::stri
     if (!physicsMaxHullSize(&max_hull_size, err)) return false;
     P.maxHullSize = max_hull_size;
     if (max_hull_size > kMinHullSizeCap) {
-        if (!alloc((void **)&P.largePairs, sizeof(PairEntry) * W * P.maxCandidatesPerWorld) ||
-            !alloc((void **)&P.largeCounts, sizeof(i32) * 3) ||
+        if (!alloc_list(P.largePairs, 2) ||
             !alloc((void **)&ph->classInfo, sizeof(i32) * 3)) {
             *err = "physics buffers allocation failed";
             return false;
@@ -3046,10 +3001,10 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
             // world order (the reference sorts Joint here too, xpbd.cpp:1092-1096).
             // Tag 1: the standalone overlap tasks, no solver reads the joints.
             if (rec.userTag != 1) launchSortArchetype(ex, ph->hPhys.jointArchetype, 1, s);
-            // the search appends the step's pairs to two empty lists
-            cudaMemsetAsync(ph->hPhys.pairCounts, 0, 2 * sizeof(i32), s);
-            // and the pairs with a hull past the staging caps to a third
-            if (ph->largeHulls) cudaMemsetAsync(ph->hPhys.largeCounts, 0, sizeof(i32), s);
+            // the search appends the step's pairs to empty lists: hull - hull, other and, with
+            // a hull past the staging caps, large (tickets are zero between launches)
+            cudaMemsetAsync(ph->hPhys.hullPairs.counters, 0,
+                            (ph->largeHulls ? 3 : 2) * sizeof(PairListCounters), s);
             physFindCandidatesKernel<<<wgrid, wblock, 0, s>>>(d);
             break;
         case NodePhysSubstepBegin:

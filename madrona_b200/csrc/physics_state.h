@@ -81,14 +81,22 @@ struct PhysicsWorldParams {
     u32 jointArchetypeID;
 };
 
+// Class of a candidate pair: the OR of its primitives' types (sphere 1, hull 2, plane 4)
+enum PairClass : u32 {
+    PairSphereSphere = 1,
+    PairHullHull = 2,
+    PairSphereHull = 3,
+    PairSpherePlane = 5,
+    PairHullPlane = 6,
+};
+
 // Role of phys::CandidateCollision (physics.hpp:52-57: two Locs + two primitive
 // indices, 24 B), resolved by the candidate search into everything about the pair
 // that stays fixed for the step, so that every substep's narrowphase only loads the
 // poses and the primitive boxes.  Side a / b are already in primitive type order
 // (sphere < hull < plane):
 //   aPrim, bPrim = indices into the world's ObjectManager::prims
-//   arch  = aArch | bArch << 8 | pair class << 16, class = aType | bType
-//           (1 sphere-sphere, 2 hull-hull, 3 sphere-hull, 5 sphere-plane, 6 hull-plane)
+//   arch  = aArch | bArch << 8 | PairClass << 16
 //   slots = aSlot | aMutable << 15 | ... same for b in the high half, i.e.
 //           ((slot << 1) | mutable) per side with slot = index of the body in
 //           its world's body list (0x7fff: unknown) and mutable = "writing the
@@ -111,6 +119,19 @@ struct alignas(16) Candidate {
 struct PairEntry {
     i32 world;
     i32 cand;
+};
+
+// A work list of the step's pairs, in any order across worlds: appended by the candidate
+// search, handed out to the narrowphase's warps by the ticket.
+struct PairListCounters {
+    i32 count;        // entries, reset before each candidate search
+    i32 ticket;       // next work item; zero between launches
+    i32 finished;     // warps of the launch that took their last ticket; zero between launches
+};
+
+struct PairList {
+    PairEntry *entries;          // [numWorlds * maxCandidatesPerWorld]
+    PairListCounters *counters;
 };
 
 // == phys::ContactConstraint (physics.hpp:59-65) + xpbd::XPBDContactState
@@ -192,14 +213,10 @@ struct PhysicsState {
     i32 *contactCounts;
     i32 *contactMaxLevel;        // [numWorlds]
     i32 maxContactsPerWorld;
-    // the step's candidates as two work lists, hull - hull pairs and all other pairs,
-    // in any order across worlds: built by the candidate search, read by every
-    // substep's narrowphase (counts reset before each search)
-    PairEntry *hullPairs;        // [numWorlds * maxCandidatesPerWorld]
-    PairEntry *otherPairs;       // [numWorlds * maxCandidatesPerWorld]
-    // [0] hull - hull, [1] other; [2], [3] the narrowphase's item ticket and
-    // finished-warp count, zero between launches
-    i32 *pairCounts;
+    // the step's candidates as two work lists, hull - hull pairs and all other pairs, read
+    // by every substep's narrowphase, which hands out the items of both by hullPairs' ticket
+    PairList hullPairs;
+    PairList otherPairs;
 
     // ---- hulls past the staging caps (MADRONA_B200_MAX_HULL_SIZE > 16)
     i32 maxHullSize;             // 16: none of the fields below is used
@@ -211,8 +228,7 @@ struct PhysicsState {
     i32 numPrimClasses;
     // the step's pairs with a large or too large primitive, of every pair type: the third
     // work list, read by physNarrowphaseLargeKernel
-    PairEntry *largePairs;       // [numWorlds * maxCandidatesPerWorld]
-    i32 *largeCounts;            // [0] pairs, [1] ticket, [2] finished warps (as pairCounts[2], [3])
+    PairList largePairs;
 };
 
 }

@@ -6,7 +6,10 @@
     from a torch.profiler trace of its own, the time of physNarrowphaseLargeKernel and of
     the group-per-pair physNarrowphaseKernel per substep;
 (b) room at 8192 worlds with the knob unset and at 255, alternating, three runs each: no
-    primitive of room is large, so both run the same kernels.
+    primitive of room is large, so both run the same kernels;
+(c) hullpile (hulls at the staging caps among balls and capped boxes) at 4096 worlds with the
+    knob unset, three runs: its spheres select the sphere - hull path of physNarrowphaseKernel,
+    which no bench.py workload runs.
 
     python scripts/bench_large_hulls.py [--steps 100] [--warmup 60]
 
@@ -89,6 +92,21 @@ def hullpile_big(worlds, knob, steps, warmup):
     return res
 
 
+def hullpile(worlds, steps, warmup):
+    from sims import make_executor
+    set_knob(None)
+    ex = make_executor("hullpile", worlds, seed=41)
+    graph = ex.buildLaunchGraphAllTaskGraphs()
+    for _ in range(warmup):        # the column falls and piles up
+        ex.run(graph)
+    ms = timed_steps(ex, graph, steps)
+    kernel = kernel_ms_per_launch(ex, graph, 20, ["physNarrowphaseKernel"])["physNarrowphaseKernel"]
+    assert kernel["launches"] == 20 * SUBSTEPS, kernel
+    del graph
+    ex.close()
+    return round(ms, 4), kernel["ms"]
+
+
 def room(worlds, knob, steps, warmup):
     import numpy as np
     import torch
@@ -120,6 +138,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=60)
     ap.add_argument("--pile-worlds", type=int, default=4096)
     ap.add_argument("--room-worlds", type=int, default=8192)
+    ap.add_argument("--sphere-worlds", type=int, default=4096)
     args = ap.parse_args()
 
     import torch
@@ -136,12 +155,15 @@ def main():
             key = "unset" if knob is None else str(knob)
             runs[key].append(round(ms, 4))
             kernels[key] = n
+    spheres = [hullpile(args.sphere_worlds, args.steps, args.warmup) for _ in range(3)]
     set_knob(None)
     print(json.dumps({
         "gpu": name, "power_limit": limit, "steps": args.steps, "warmup": args.warmup,
         "hullpile_big": pile,
         "room": {"worlds": args.room_worlds, "ms_per_step": runs, "kernels_in_graph": kernels,
-                 "mean_ms_per_step": {k: round(sum(v) / len(v), 4) for k, v in runs.items()}}}))
+                 "mean_ms_per_step": {k: round(sum(v) / len(v), 4) for k, v in runs.items()}},
+        "hullpile": {"worlds": args.sphere_worlds, "ms_per_step": [ms for ms, _ in spheres],
+                     "narrowphase_ms_per_substep": [k for _, k in spheres]}}))
 
 
 if __name__ == "__main__":
