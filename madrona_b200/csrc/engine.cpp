@@ -371,10 +371,10 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
     }
 
     {
-        // so is the hull-size knob of the physics narrowphase
-        int max_hull_size;
+        // so are the hull-size and world-size knobs of the physics
+        int max_hull_size, max_world_bodies;
         std::string err;
-        if (!physicsMaxHullSize(&max_hull_size, &err)) {
+        if (!physicsMaxHullSize(&max_hull_size, &err) || !physicsMaxWorldBodies(&max_world_bodies, &err)) {
             setError(err);
             return false;
         }

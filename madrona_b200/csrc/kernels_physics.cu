@@ -86,6 +86,8 @@ struct PhysicsHost {
     bool largeHulls = false;         // some primitive needs the warp-per-pair kernel (read before graph capture)
     unsigned largeBlocks = 0;        // its persistent grid (0: it does not fit / the query failed)
     std::string largeError;          // why a launch graph with physics cannot be built
+    // worlds past 128 bodies (MADRONA_B200_MAX_BODIES_PER_WORLD > 128)
+    unsigned largeSearchBlocks = 0;  // persistent grid of physFindCandidatesLargeKernel (0: query failed)
 };
 
 // ---- small device helpers ------------------------------------------------------------
@@ -299,7 +301,12 @@ __device__ i32 midpointPartition(WorldBVH &bvh, i32 base, i32 n)
     return (lo > 0 && lo < n) ? lo : n / 2;
 }
 
-__device__ void rebuildWorldBVH(WorldBVH &bvh)
+// Both stacks of the build hold 64 entries, as the reference's (broadphase.cpp:60).  A tree
+// too deep for them (clustered leaves make the midpoint splits lopsided) is not built:
+// returns false with numTraversal = 0, so no search or query reads a partial leaf list.
+constexpr int kRebuildStack = 64;
+
+__device__ bool rebuildWorldBVH(WorldBVH &bvh)
 {
     const i32 num_leaves = bvh.numLeaves;
     i32 third = (num_leaves - 1 + 2) / 3;
@@ -311,7 +318,7 @@ __device__ void rebuildWorldBVH(WorldBVH &bvh)
         i32 offset;
         i32 count;
     };
-    Pending stack[64];
+    Pending stack[kRebuildStack];
     stack[0] = Pending { -1, -1, 0, num_leaves };
     i32 depth = 1;
     i32 next_node = 0;
@@ -341,6 +348,10 @@ __device__ void rebuildWorldBVH(WorldBVH &bvh)
         } else if (top.node == -1) {
             // first visit of an inner entry: take a node, split the range into
             // quarters (half, then each half again) and descend left to right
+            if (depth + 4 > kRebuildStack) {
+                bvh.numTraversal = 0;
+                return false;
+            }
             node_id = next_node++;
             top.node = node_id;
             BVHNode &node = bvh.nodes[node_id];
@@ -382,7 +393,7 @@ __device__ void rebuildWorldBVH(WorldBVH &bvh)
 
     // report order of an un-pruned traversal (include/madrona/broadphase.inl:21-59)
     i32 order_n = 0;
-    i32 walk[64];
+    i32 walk[kRebuildStack];
     walk[0] = 0;
     i32 walk_n = 1;
     while (walk_n > 0) {
@@ -392,8 +403,11 @@ __device__ void rebuildWorldBVH(WorldBVH &bvh)
             if (child == -1) continue;
             if (child & 0x80000000) {
                 if (order_n < bvh.numAllocatedLeaves) bvh.traversalOrder[order_n++] = child & 0x7fffffff;
-            } else if (walk_n < 64) {
+            } else if (walk_n < kRebuildStack) {
                 walk[walk_n++] = child;
+            } else {
+                bvh.numTraversal = 0;
+                return false;
             }
         }
     }
@@ -407,18 +421,22 @@ __device__ void rebuildWorldBVH(WorldBVH &bvh)
         bvh.orderedBoxes[2 * k] = PVec4 { node.minX[sub], node.minY[sub], node.minZ[sub], node.maxX[sub] };
         bvh.orderedBoxes[2 * k + 1] = PVec4 { node.maxY[sub], node.maxZ[sub], __int_as_float(leaf), 0.f };
     }
+    return true;
 }
 
 __device__ void refitLeaf(WorldBVH &bvh, i32 leaf);
 
 // Rebuild (rare: after a reset) followed by the refit of every leaf of the
 // world, which the fused update+refit kernel skipped for this world.
-__device__ __forceinline__ void phaseRebuild(const EngineState &S, const PhysicsState &P, const i32 w)
+__device__ __forceinline__ void phaseRebuild(EngineState &S, const PhysicsState &P, const i32 w)
 {
     WorldBVH &bvh = worldBVH(S, P, w);
     if (!bvh.forceRebuild) return;
     bvh.forceRebuild = 0;
-    rebuildWorldBVH(bvh);
+    if (!rebuildWorldBVH(bvh)) {
+        atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);   // the tree is deeper than the build's stacks
+        return;
+    }
     for (u32 bi = 0; bi < P.numBodyArchetypes; bi++) {
         const BodyArchetype &b = P.bodies[bi];
         const TableDesc &t = S.tables[b.archetype];
@@ -550,12 +568,163 @@ __device__ __forceinline__ void appendPairs(const PairList &list, const bool tak
     if (take) list.entries[at + __popc(mask & ((1u << lane) - 1u))] = PairEntry { w, i };
 }
 
+// The rules of the candidate search.  Two kernels search: one warp per world for worlds of
+// up to kMaxStagedLeaves leaves (phaseFindCandidates) and one block per world for larger
+// ones (phaseFindCandidatesLarge).  Both describe leaves and bodies, test pairs, write
+// candidates and fill the step's work lists through the helpers below and differ only in
+// how the work is spread and where the staged leaves live, so both emit the same list.
+
+// (world body slot << 1) | mutable of a body (Candidate::slots)
+__device__ __forceinline__ u32 bodySlotInfo(const EngineState &S, const PhysicsState &P, const i32 w,
+                                            const u32 arch, const i32 row, const bool is_static)
+{
+    const i32 slot = worldBodySlot(S, P, w, arch, row);
+    bool is_mutable = true;
+    if (is_static) is_mutable = !rotationIsNormalizeFixpoint(cachedCol<Quat>(arch, PCRotation, row));
+    const u32 s15 = (slot < 0 || slot >= (i32)kUnknownSlot) ? kUnknownSlot : (u32)slot;
+    return (s15 << 1) | (is_mutable ? 1u : 0u);
+}
+
+// The k-th leaf the world's tree reports, as a partner
+__device__ __forceinline__ StagedLeaf describeLeaf(EngineState &S, const PhysicsState &P, const i32 w,
+                                                   const WorldBVH &bvh, const ObjectManager &objs, const i32 k)
+{
+    const float4 b0 = reinterpret_cast<const float4 *>(bvh.orderedBoxes)[2 * k];
+    const float4 b1 = reinterpret_cast<const float4 *>(bvh.orderedBoxes)[2 * k + 1];
+    const i32 leaf = __float_as_int(b1.z);
+    StagedLeaf sl;
+    sl.box[0] = b0.x; sl.box[1] = b0.y; sl.box[2] = b0.z;
+    sl.box[3] = b0.w; sl.box[4] = b1.x; sl.box[5] = b1.y;
+    const u64 packed = bvh.leafEntities[leaf];
+    sl.entityID = (i32)(u32)(packed >> 32);
+    const u32 gen = (u32)(packed & 0xFFFFFFFFull);
+    sl.arch = 0; sl.row = 0; sl.prims = 0; sl.primBase = 0; sl.isStatic = 0; sl.slotInfo = 0;
+    if (sl.entityID >= 0 && sl.entityID < S.entityCapacity) {
+        const EntitySlot es = S.entitySlots[sl.entityID];
+        const BodyArchetype *bb = es.gen == gen ? bodyOf(P, (u32)es.a) : nullptr;
+        if (bb) {
+            sl.arch = (u32)es.a;
+            sl.row = es.b;
+            sl.isStatic = bodyCol<u32>(S, *bb, PCResponseType, es.b) == kRespStatic ? 1u : 0u;
+            const i32 obj = bodyCol<i32>(S, *bb, PCObjectID, es.b);
+            sl.prims = objs.primCounts[obj];
+            sl.primBase = objs.primOffsets[obj];
+            sl.slotInfo = bodySlotInfo(S, P, w, sl.arch, sl.row, sl.isStatic != 0);
+            if (sl.arch > 0xffu || sl.prims > 0xffu) {
+                atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);   // does not fit the packed candidate
+                sl.prims = 0;
+            }
+        }
+    }
+    return sl;
+}
+
+// The iterating body: row `row` of body archetype b (valid: the row is one of world w's)
+struct SearchBody {
+    i32 id;
+    bool isStatic;
+    u32 prims;
+    u32 primBase;
+    u32 info;           // bodySlotInfo
+    AABB box;           // its leaf box
+};
+
+__device__ __forceinline__ SearchBody describeBody(EngineState &S, const PhysicsState &P, const i32 w,
+                                                   const WorldBVH &bvh, const ObjectManager &objs,
+                                                   const BodyArchetype &b, const i32 row, const bool valid)
+{
+    SearchBody sb;
+    sb.id = 0;
+    sb.isStatic = false;
+    sb.prims = 0;
+    sb.primBase = 0;
+    sb.info = 0;
+    sb.box = AABB::invalid();
+    if (valid) {
+        const TableDesc &t = S.tables[b.archetype];
+        const u64 packed = ((const u64 *)t.columns[0])[row];
+        sb.id = (i32)(u32)(packed >> 32);
+        sb.isStatic = bodyCol<u32>(S, b, PCResponseType, row) == kRespStatic;
+        const i32 obj = bodyCol<i32>(S, b, PCObjectID, row);
+        sb.prims = objs.primCounts[obj];
+        sb.primBase = objs.primOffsets[obj];
+        sb.info = bodySlotInfo(S, P, w, b.archetype, row, sb.isStatic);
+        if (b.archetype > 0xffu || sb.prims > 0xffu) {
+            atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
+            sb.prims = 0;
+        }
+        const PAABB lb = bvh.leafAABBs[bodyCol<i32>(S, b, PCLeafID, row)];
+        sb.box = AABB { { lb.pMin.x, lb.pMin.y, lb.pMin.z }, { lb.pMax.x, lb.pMax.y, lb.pMax.z } };
+    }
+    return sb;
+}
+
+// The reference reports the leaf for the body and visits the pair: the body iterates (the
+// smaller entity ID) and the two are not both static
+__device__ __forceinline__ bool pairsWith(const SearchBody &sb, const bool valid, const StagedLeaf &sl)
+{
+    const AABB other { { sl.box[0], sl.box[1], sl.box[2] }, { sl.box[3], sl.box[4], sl.box[5] } };
+    return valid && sl.prims != 0 && sb.box.overlaps(other) && sb.id < sl.entityID && !(sb.isStatic && sl.isStatic);
+}
+
+// Check c of the pair (body, leaf), c in [0, sb.prims * sl.prims): primitive c / sl.prims of
+// the body against primitive c % sl.prims of the leaf.
+// Resolved once per step: no user node runs inside the physics chain, so ObjectID and the
+// primitive tables stay as they are until the last substep.  Order the pair by primitive
+// type: sphere(1) < hull(2) < plane(4)
+__device__ __forceinline__ Candidate pairCandidate(const ObjectManager &objs, const SearchBody &sb,
+                                                   const u32 arch, const i32 row, const StagedLeaf &sl,
+                                                   const u32 c)
+{
+    const u32 a_rel = c / sl.prims, b_rel = c % sl.prims;
+    const u32 a_prim = sb.primBase + a_rel, b_prim = sl.primBase + b_rel;
+    const u32 ta = objs.prims[a_prim].type, tb = objs.prims[b_prim].type;
+    const u32 cls = (ta | tb) << 16;      // the PairClass
+    const u32 rel = a_rel | (b_rel << 8) | (ta > tb ? 1u << 16 : 0u);
+    return ta > tb
+        ? Candidate { b_prim, a_prim, sl.row, row, sl.arch | (arch << 8) | cls,
+                      sl.slotInfo | (sb.info << 16), { rel, 0 } }
+        : Candidate { a_prim, b_prim, row, sl.row, arch | (sl.arch << 8) | cls,
+                      sb.info | (sl.slotInfo << 16), { rel, 0 } };
+}
+
+// The step's work lists, hull - hull pairs and the others (one atomic per warp, list and 32
+// candidates); with a primitive class table, the pairs of any type that have a hull past the
+// staging caps go to a third list instead.  The warp takes the world's candidates
+// [first, first + 32), [first + stride, ...) up to `running`, all its lanes together.
+__device__ __forceinline__ void appendWorldPairs(const PhysicsState &P, const Candidate *out, const i32 w,
+                                                 const i32 running, const i32 first, const i32 stride,
+                                                 const int lane)
+{
+    const unsigned char *const prim_class = P.primClass;     // uniform for the launch
+    for (i32 base = first; base < running; base += stride) {
+        const i32 i = base + lane;
+        bool valid = i < running;
+        if (prim_class) {
+            bool large = false;
+            if (valid) {
+                const u32 pa = out[i].aPrim, pb = out[i].bPrim;
+                const u32 n = (u32)P.numPrimClasses;
+                large = (pa < n ? prim_class[pa] : (u32)PrimTooLarge) != PrimSmall ||
+                        (pb < n ? prim_class[pb] : (u32)PrimTooLarge) != PrimSmall;
+            }
+            appendPairs(P.largePairs, large, w, i, lane);
+            valid = valid && !large;
+        }
+        const bool hh = valid && (out[i].arch >> 16) == PairHullHull;
+        appendPairs(P.hullPairs, hh, w, i, lane);
+        appendPairs(P.otherPairs, valid && !hh, w, i, lane);
+    }
+}
+
 // Candidate pairs of one world, in the CPU backend's order (bodies: archetype
 // ascending, then row; partners of a body: BVH report order).  The set a
 // traversal reports for body a is { leaf b : slotBox(b) overlaps leafBox(a) }
 // (ancestor boxes contain their leaves' slot boxes, so pruning removes nothing
 // else) and its order is the tree's fixed report order, so the search is a
 // uniform loop over the staged leaves instead of 32 divergent stack walks.
+// A world of more than kMaxStagedLeaves leaves, up to PhysicsState::maxWorldBodies, goes to
+// the large-world list for phaseFindCandidatesLarge instead; past that it raises.
 __device__ void phaseFindCandidates(EngineState &S, const PhysicsState &P, const i32 w, const int lane,
                                     const int warp, CandidateScratch &scratch)
 {
@@ -568,49 +737,18 @@ __device__ void phaseFindCandidates(EngineState &S, const PhysicsState &P, const
     const i32 num_leaves = bvh.numTraversal;
     if (num_leaves > kMaxStagedLeaves) {
         if (lane == 0) {
-            atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
-            P.candCounts[w] = 0;
+            if (num_leaves <= P.maxWorldBodies) {
+                const i32 at = atomicAdd(&P.largeWorlds.counters->count, 1);
+                P.largeWorlds.entries[at] = PairEntry { w, num_leaves };
+            } else {
+                atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
+                P.candCounts[w] = 0;
+            }
         }
         return;
     }
-    auto bodySlotInfo = [&](u32 arch, i32 row, bool is_static) -> u32 {
-        const i32 slot = worldBodySlot(S, P, w, arch, row);
-        bool is_mutable = true;
-        if (is_static) is_mutable = !rotationIsNormalizeFixpoint(cachedCol<Quat>(arch, PCRotation, row));
-        const u32 s15 = (slot < 0 || slot >= (i32)kUnknownSlot) ? kUnknownSlot : (u32)slot;
-        return (s15 << 1) | (is_mutable ? 1u : 0u);
-    };
     // stage 1: lane k describes the k-th reported leaf
-    for (i32 k = lane; k < num_leaves; k += 32) {
-        const float4 b0 = reinterpret_cast<const float4 *>(bvh.orderedBoxes)[2 * k];
-        const float4 b1 = reinterpret_cast<const float4 *>(bvh.orderedBoxes)[2 * k + 1];
-        const i32 leaf = __float_as_int(b1.z);
-        StagedLeaf sl;
-        sl.box[0] = b0.x; sl.box[1] = b0.y; sl.box[2] = b0.z;
-        sl.box[3] = b0.w; sl.box[4] = b1.x; sl.box[5] = b1.y;
-        const u64 packed = bvh.leafEntities[leaf];
-        sl.entityID = (i32)(u32)(packed >> 32);
-        const u32 gen = (u32)(packed & 0xFFFFFFFFull);
-        sl.arch = 0; sl.row = 0; sl.prims = 0; sl.primBase = 0; sl.isStatic = 0; sl.slotInfo = 0;
-        if (sl.entityID >= 0 && sl.entityID < S.entityCapacity) {
-            const EntitySlot es = S.entitySlots[sl.entityID];
-            const BodyArchetype *bb = es.gen == gen ? bodyOf(P, (u32)es.a) : nullptr;
-            if (bb) {
-                sl.arch = (u32)es.a;
-                sl.row = es.b;
-                sl.isStatic = bodyCol<u32>(S, *bb, PCResponseType, es.b) == kRespStatic ? 1u : 0u;
-                const i32 obj = bodyCol<i32>(S, *bb, PCObjectID, es.b);
-                sl.prims = objs.primCounts[obj];
-                sl.primBase = objs.primOffsets[obj];
-                sl.slotInfo = bodySlotInfo(sl.arch, sl.row, sl.isStatic != 0);
-                if (sl.arch > 0xffu || sl.prims > 0xffu) {
-                    atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);   // does not fit the packed candidate
-                    sl.prims = 0;
-                }
-            }
-        }
-        staged[k] = sl;
-    }
+    for (i32 k = lane; k < num_leaves; k += 32) staged[k] = describeLeaf(S, P, w, bvh, objs, k);
     __syncwarp();
 
     for (u32 bi = 0; bi < P.numBodyArchetypes; bi++) {
@@ -621,28 +759,7 @@ __device__ void phaseFindCandidates(EngineState &S, const PhysicsState &P, const
         for (i32 base = 0; base < count; base += 32) {
             const i32 row = first + base + lane;
             const bool valid = base + lane < count && ((const i32 *)t.columns[1])[row] == w;
-
-            i32 self_id = 0;
-            bool self_static = false;
-            u32 self_prims = 0;
-            u32 self_base = 0;
-            u32 self_info = 0;
-            AABB box = AABB::invalid();
-            if (valid) {
-                const u64 packed = ((const u64 *)t.columns[0])[row];
-                self_id = (i32)(u32)(packed >> 32);
-                self_static = bodyCol<u32>(S, b, PCResponseType, row) == kRespStatic;
-                const i32 obj = bodyCol<i32>(S, b, PCObjectID, row);
-                self_prims = objs.primCounts[obj];
-                self_base = objs.primOffsets[obj];
-                self_info = bodySlotInfo(b.archetype, row, self_static);
-                if (b.archetype > 0xffu || self_prims > 0xffu) {
-                    atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
-                    self_prims = 0;
-                }
-                const PAABB lb = bvh.leafAABBs[bodyCol<i32>(S, b, PCLeafID, row)];
-                box = AABB { { lb.pMin.x, lb.pMin.y, lb.pMin.z }, { lb.pMax.x, lb.pMax.y, lb.pMax.z } };
-            }
+            const SearchBody sb = describeBody(S, P, w, bvh, objs, b, row, valid);
 
             // stage 2: which staged leaves does this body pair with (bit k of word k / 64)
             unsigned long long partners[kLeafMaskWords];
@@ -654,12 +771,9 @@ __device__ void phaseFindCandidates(EngineState &S, const PhysicsState &P, const
                 const i32 k_end = min(num_leaves, (wd + 1) * 64);
                 for (i32 k = wd * 64; k < k_end; k++) {
                     const StagedLeaf &sl = staged[k];
-                    const AABB other { { sl.box[0], sl.box[1], sl.box[2] }, { sl.box[3], sl.box[4], sl.box[5] } };
-                    const bool pair = valid && sl.prims != 0 && box.overlaps(other) &&
-                        self_id < sl.entityID && !(self_static && sl.isStatic);
-                    if (pair) {
+                    if (pairsWith(sb, valid, sl)) {
                         partners[wd] |= 1ull << (k - wd * 64);
-                        mine += (i32)(self_prims * sl.prims);
+                        mine += (i32)(sb.prims * sl.prims);
                     }
                 }
             }
@@ -678,24 +792,9 @@ __device__ void phaseFindCandidates(EngineState &S, const PhysicsState &P, const
                     const int k = wd * 64 + __ffsll((long long)word) - 1;
                     word &= word - 1;
                     const StagedLeaf &sl = staged[k];
-                    const u32 checks = self_prims * sl.prims;
+                    const u32 checks = sb.prims * sl.prims;
                     for (u32 c = 0; c < checks; c++) {
-                        if (at < P.maxCandidatesPerWorld) {
-                            // Resolved once per step: no user node runs inside the physics
-                            // chain, so ObjectID and the primitive tables stay as they are
-                            // until the last substep.  Order the pair by primitive type:
-                            // sphere(1) < hull(2) < plane(4)
-                            const u32 a_rel = c / sl.prims, b_rel = c % sl.prims;
-                            const u32 a_prim = self_base + a_rel, b_prim = sl.primBase + b_rel;
-                            const u32 ta = objs.prims[a_prim].type, tb = objs.prims[b_prim].type;
-                            const u32 cls = (ta | tb) << 16;      // the PairClass
-                            const u32 rel = a_rel | (b_rel << 8) | (ta > tb ? 1u << 16 : 0u);
-                            out[at] = ta > tb
-                                ? Candidate { b_prim, a_prim, sl.row, row, sl.arch | (b.archetype << 8) | cls,
-                                              sl.slotInfo | (self_info << 16), { rel, 0 } }
-                                : Candidate { a_prim, b_prim, row, sl.row, b.archetype | (sl.arch << 8) | cls,
-                                              self_info | (sl.slotInfo << 16), { rel, 0 } };
-                        }
+                        if (at < P.maxCandidatesPerWorld) out[at] = pairCandidate(objs, sb, b.archetype, row, sl, c);
                         at++;
                     }
                 }
@@ -709,29 +808,115 @@ __device__ void phaseFindCandidates(EngineState &S, const PhysicsState &P, const
     }
     if (lane == 0) P.candCounts[w] = running;
 
-    // the step's work lists, hull - hull pairs and the others (one atomic per warp, list
-    // and 32 candidates); with a primitive class table, the pairs of any type that have a
-    // hull past the staging caps go to a third list instead
     __syncwarp();
-    const unsigned char *const prim_class = P.primClass;     // uniform for the launch
-    for (i32 base = 0; base < running; base += 32) {
-        const i32 i = base + lane;
-        bool valid = i < running;
-        if (prim_class) {
-            bool large = false;
-            if (valid) {
-                const u32 pa = out[i].aPrim, pb = out[i].bPrim;
-                const u32 n = (u32)P.numPrimClasses;
-                large = (pa < n ? prim_class[pa] : (u32)PrimTooLarge) != PrimSmall ||
-                        (pb < n ? prim_class[pb] : (u32)PrimTooLarge) != PrimSmall;
+    appendWorldPairs(P, out, w, running, 0, 32, lane);
+}
+
+// ---- candidate pairs of worlds past kMaxStagedLeaves leaves: one block per world -----------
+// The same flat scan in the same order, spread over a block: thread t describes body
+// base + t of the world's body list (archetypes ascending, rows in order), the reported
+// leaves are staged kLargeSearchTile at a time in shared memory, a count pass over all
+// tiles gives each body its number of checks, a block-wide exclusive scan in body order its
+// emission offset, and an emit pass over the tiles writes its candidates in report order.
+// Every leaf is tested against every body twice: O(N^2) per world.
+constexpr int kLargeSearchThreads = 256;
+constexpr int kLargeSearchWarps = kLargeSearchThreads / 32;
+constexpr int kLargeSearchTile = 512;
+
+struct LargeSearchScratch {
+    StagedLeaf tile[kLargeSearchTile];
+    long long warpSums[kLargeSearchWarps];
+    i32 ticket;
+};
+
+__device__ __forceinline__ void stageLeafTile(EngineState &S, const PhysicsState &P, const i32 w,
+                                              const WorldBVH &bvh, const ObjectManager &objs,
+                                              LargeSearchScratch &sh, const i32 first, const i32 n)
+{
+    __syncthreads();      // the previous tile is no longer read
+    for (i32 k = threadIdx.x; k < n; k += kLargeSearchThreads) sh.tile[k] = describeLeaf(S, P, w, bvh, objs, first + k);
+    __syncthreads();
+}
+
+__device__ __forceinline__ void phaseFindCandidatesLarge(EngineState &S, const PhysicsState &P, const i32 w,
+                                                         LargeSearchScratch &sh)
+{
+    const WorldBVH &bvh = worldBVH(S, P, w);
+    const ObjectManager &objs = *(const ObjectManager *)bvh.objMgr;
+    Candidate *out = P.candidates + (size_t)w * P.maxCandidatesPerWorld;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const i32 num_leaves = bvh.numTraversal;
+    const long long max_cands = P.maxCandidatesPerWorld;
+    long long running = 0;     // no wrap-around before the cap check, whatever the world holds
+    i32 staged_first = -1;     // first leaf of the tile in shared memory
+
+    for (u32 bi = 0; bi < P.numBodyArchetypes; bi++) {
+        const BodyArchetype &b = P.bodies[bi];
+        const TableDesc &t = S.tables[b.archetype];
+        const i32 first = t.worldOffsets[w];
+        const i32 count = t.worldCounts[w];
+        for (i32 base = 0; base < count; base += kLargeSearchThreads) {
+            const i32 row = first + base + tid;
+            const bool valid = base + tid < count && ((const i32 *)t.columns[1])[row] == w;
+            const SearchBody sb = describeBody(S, P, w, bvh, objs, b, row, valid);
+
+            // count pass
+            long long mine = 0;
+            for (i32 t0 = 0; t0 < num_leaves; t0 += kLargeSearchTile) {
+                const i32 n = min(kLargeSearchTile, num_leaves - t0);
+                if (t0 != staged_first) {
+                    stageLeafTile(S, P, w, bvh, objs, sh, t0, n);
+                    staged_first = t0;
+                }
+                for (i32 k = 0; k < n; k++) {
+                    const StagedLeaf &sl = sh.tile[k];
+                    if (pairsWith(sb, valid, sl)) mine += (long long)(sb.prims * sl.prims);
+                }
             }
-            appendPairs(P.largePairs, large, w, i, lane);
-            valid = valid && !large;
+            // exclusive scan over the block = emission offsets in body order
+            long long incl = mine;
+            for (int o = 1; o < 32; o <<= 1) {
+                const long long up = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += up;
+            }
+            if (lane == 31) sh.warpSums[warp] = incl;
+            __syncthreads();
+            long long before = 0, total = 0;
+            for (int i = 0; i < kLargeSearchWarps; i++) {
+                const long long s = sh.warpSums[i];
+                if (i < warp) before += s;
+                total += s;
+            }
+            long long at = running + before + incl - mine;
+
+            // emit pass: the tiles again, in report order
+            for (i32 t0 = 0; t0 < num_leaves; t0 += kLargeSearchTile) {
+                const i32 n = min(kLargeSearchTile, num_leaves - t0);
+                if (t0 != staged_first) {
+                    stageLeafTile(S, P, w, bvh, objs, sh, t0, n);
+                    staged_first = t0;
+                }
+                for (i32 k = 0; k < n && mine != 0; k++) {
+                    const StagedLeaf &sl = sh.tile[k];
+                    if (!pairsWith(sb, valid, sl)) continue;
+                    const u32 checks = sb.prims * sl.prims;
+                    for (u32 c = 0; c < checks && at < max_cands; c++, at++) {
+                        out[at] = pairCandidate(objs, sb, b.archetype, row, sl, c);
+                    }
+                }
+            }
+            running += total;
+            __syncthreads();   // warpSums is read by all before the next body chunk writes it
         }
-        const bool hh = valid && (out[i].arch >> 16) == PairHullHull;
-        appendPairs(P.hullPairs, hh, w, i, lane);
-        appendPairs(P.otherPairs, valid && !hh, w, i, lane);
     }
+    if (running > max_cands) {
+        if (tid == 0) atomicOr(&S.errorFlags, (u32)ErrPhysicsOverflow);
+        running = max_cands;
+    }
+    if (tid == 0) P.candCounts[w] = (i32)running;
+
+    __syncthreads();   // the block's candidates are written before its warps list them
+    appendWorldPairs(P, out, w, (i32)running, warp * 32, kLargeSearchThreads, lane);
 }
 
 // =============================================================================================
@@ -1918,7 +2103,11 @@ physClassifyPrimsKernel(EngineState *Sp, unsigned char *classes, i32 num_prims, 
 // Prologue of the position solve, run by the LPW lanes that own world w: list
 // the world's contact slots in candidate order and give every contact its
 // dependency level (see Contact::level) -- a sequential scan by the group's
-// first lane over flags / body infos its lanes fetched in parallel.
+// first lane over flags / body infos its lanes fetched in parallel.  The last level of
+// each body slot is kept in `last_level` (shared, kMaxLevelBodies slots), or, for a world
+// with more body slots when PhysicsState::levelScratch exists, in the world's row of it
+// (up to maxWorldBodies slots).  A contact on a slot past the table is ordered after
+// everything before it.
 template <int LPW>
 __device__ __forceinline__ void orderContacts(EngineState &S, const PhysicsState &P, const i32 w, const bool valid,
                                               const int lane, i32 *last_level /* [kMaxLevelBodies] of this world */)
@@ -1928,7 +2117,16 @@ __device__ __forceinline__ void orderContacts(EngineState &S, const PhysicsState
     const int group_shift = (lane / LPW) * LPW;
     const unsigned gm = kGroupMask << group_shift;
 
-    for (int i = sub; i < kMaxLevelBodies; i += LPW) last_level[i] = 0;
+    i32 num_slots = kMaxLevelBodies;
+    if (P.levelScratch && valid) {
+        i32 bodies = 0;
+        for (u32 bi = 0; bi < P.numBodyArchetypes; bi++) bodies += S.tables[P.bodies[bi].archetype].worldCounts[w];
+        if (bodies > kMaxLevelBodies) {
+            last_level = P.levelScratch + (size_t)w * P.maxWorldBodies;
+            num_slots = min(bodies, P.maxWorldBodies);
+        }
+    }
+    for (int i = sub; i < num_slots; i += LPW) last_level[i] = 0;
     __syncwarp(gm);
 
     const i32 n = valid ? P.candCounts[w] : 0;
@@ -1956,7 +2154,7 @@ __device__ __forceinline__ void orderContacts(EngineState &S, const PhysicsState
             i32 lvl = 0;
             if (sub == 0) {
                 const u32 sa = sa_info >> 1, sb = sb_info >> 1;
-                if (sa >= (u32)kMaxLevelBodies || sb >= (u32)kMaxLevelBodies) {
+                if (sa >= (u32)num_slots || sb >= (u32)num_slots) {
                     lvl = max_level + 1;          // unknown body: strictly after everything so far
                     seq_level = lvl;
                 } else {
@@ -2570,7 +2768,7 @@ physBodyKernel(EngineState *Sp)
 __global__ void __launch_bounds__(128)
 physRebuildKernel(EngineState *Sp)
 {
-    const EngineState &S = *Sp;
+    EngineState &S = *Sp;
     const i32 w = blockIdx.x * blockDim.x + threadIdx.x;
     if (w >= (i32)S.numWorlds) return;
     phaseRebuild(S, *S.physics, w);
@@ -2592,6 +2790,41 @@ physFindCandidatesKernel(EngineState *Sp)
     if (w >= (i32)S.numWorlds) return;
     __shared__ CandidateScratch cand_scratch;
     phaseFindCandidates(S, P, w, lane, warp, cand_scratch);
+}
+
+// forEachTicket for a whole block: thread 0 draws the tickets, every thread runs run(item)
+// and the block syncs before the next item, which may reuse its shared memory.
+template <typename Run>
+__device__ __forceinline__ void forEachBlockTicket(PairListCounters *c, const i32 items, i32 *slot, Run &&run)
+{
+    if (threadIdx.x == 0) *slot = atomicAdd(&c->ticket, 1);
+    __syncthreads();
+    i32 item = *slot;
+    while (item < items) {
+        __syncthreads();     // every thread has read the slot
+        if (threadIdx.x == 0) *slot = atomicAdd(&c->ticket, 1);    // in flight while this item runs
+        run(item);
+        __syncthreads();
+        item = *slot;
+    }
+    if (threadIdx.x == 0 && atomicAdd(&c->finished, 1) == (i32)gridDim.x - 1) {
+        c->ticket = 0;
+        c->finished = 0;
+    }
+}
+
+// Launched right after physFindCandidatesKernel when MADRONA_B200_MAX_BODIES_PER_WORLD > 128:
+// a persistent grid over the worlds that kernel listed, one block per world.
+__global__ void __launch_bounds__(kLargeSearchThreads, 1)
+physFindCandidatesLargeKernel(EngineState *Sp)
+{
+    EngineState &S = *Sp;
+    const PhysicsState &P = *S.physics;
+    fillColCache(S, P);
+    __shared__ LargeSearchScratch scratch;
+    forEachBlockTicket(P.largeWorlds.counters, P.largeWorlds.counters->count, &scratch.ticket, [&](const i32 item) {
+        phaseFindCandidatesLarge(S, P, P.largeWorlds.entries[item].world, scratch);
+    });
 }
 
 // kSolverLanes lanes per world.  The lanes of a warp past the last world idle along
@@ -2784,6 +3017,22 @@ bool physicsMaxHullSize(int *size, std::string *err)
     return true;
 }
 
+bool physicsMaxWorldBodies(int *bodies, std::string *err)
+{
+    *bodies = kMinWorldBodiesCap;
+    const char *v = getenv("MADRONA_B200_MAX_BODIES_PER_WORLD");
+    if (!v) return true;
+    char *end = nullptr;
+    const long n = strtol(v, &end, 10);
+    if (!*v || *end != '\0' || n < kMinWorldBodiesCap || n > kMaxWorldBodiesCap) {
+        *err = "MADRONA_B200_MAX_BODIES_PER_WORLD must be a number from " + std::to_string(kMinWorldBodiesCap) +
+               " to " + std::to_string(kMaxWorldBodiesCap) + " (rigid bodies per world), got \"" + v + "\"";
+        return false;
+    }
+    *bodies = (int)n;
+    return true;
+}
+
 static size_t largeStageBytes(int max_hull_size)
 {
     return (size_t)kLargeWarps * max_hull_size * kLargeStageBytesPerEntry;
@@ -2833,8 +3082,8 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::stri
         cudaMemset(*p, 0, bytes);
         return true;
     };
-    // The step's work lists.  Their counters are one array, hull - hull, other, large, so
-    // one memset before the candidate search resets the lists a step uses.
+    // The step's work lists.  Their counters are one array, hull - hull, other, large pairs,
+    // large worlds, so one memset before the candidate search resets the lists a step uses.
     PairListCounters *pair_counters = nullptr;
     auto alloc_list = [&](PairList &list, int k) {
         list.counters = pair_counters + k;
@@ -2845,7 +3094,7 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::stri
         !alloc((void **)&P.contacts, sizeof(Contact) * W * P.maxCandidatesPerWorld) ||
         !alloc((void **)&P.candHit, sizeof(i32) * W * P.maxCandidatesPerWorld) ||
         !alloc((void **)&P.contactOrder, sizeof(i32) * W * P.maxContactsPerWorld) ||
-        !alloc((void **)&pair_counters, sizeof(PairListCounters) * 3) ||
+        !alloc((void **)&pair_counters, sizeof(PairListCounters) * 4) ||
         !alloc_list(P.hullPairs, 0) ||
         !alloc_list(P.otherPairs, 1) ||
         !alloc((void **)&P.contactCounts, sizeof(i32) * W) ||
@@ -2867,6 +3116,19 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::stri
                                  (int)largeStageBytes(max_hull_size)) != cudaSuccess) {
             cudaGetLastError();
             *err = "the large-hull narrowphase's shared memory (MADRONA_B200_MAX_HULL_SIZE) does not fit the device";
+            return false;
+        }
+    }
+    // worlds past 128 bodies: their work list and the global contact level table (4 bytes per
+    // world and body slot)
+    int max_world_bodies = kMinWorldBodiesCap;
+    if (!physicsMaxWorldBodies(&max_world_bodies, err)) return false;
+    P.maxWorldBodies = max_world_bodies;
+    if (max_world_bodies > kMinWorldBodiesCap) {
+        P.largeWorlds.counters = pair_counters + 3;
+        if (!alloc((void **)&P.largeWorlds.entries, sizeof(PairEntry) * W) ||
+            !alloc((void **)&P.levelScratch, sizeof(i32) * W * max_world_bodies)) {
+            *err = "physics buffers allocation failed";
             return false;
         }
     }
@@ -2947,6 +3209,15 @@ void physicsBeforeGraphCapture(Executor *ex)
         : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, physNarrowphaseKernel<false>, kNarrowThreads, 0);
     if (e != cudaSuccess) cudaGetLastError();
     ph->narrowBlocks = e == cudaSuccess ? (unsigned)ex->numSMs * (unsigned)per_sm : 0u;
+    if (ph->hPhys.maxWorldBodies > kMinWorldBodiesCap) {
+        per_sm = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, physFindCandidatesLargeKernel,
+                                                          kLargeSearchThreads, 0) != cudaSuccess) {
+            cudaGetLastError();
+            per_sm = 0;
+        }
+        ph->largeSearchBlocks = (unsigned)ex->numSMs * (unsigned)per_sm;
+    }
     physicsClassifyPrims(ex);
 }
 
@@ -2986,6 +3257,7 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
     const unsigned worlds_per_block = wblock / kSolverLanes;
     const unsigned sgrid = (W + worlds_per_block - 1) / worlds_per_block;
     const dim3 bgrid = bodyGrid(ex);
+    const bool large_worlds = ph->hPhys.maxWorldBodies > kMinWorldBodiesCap;
     for (uint32_t i = 0; i < count; i++) {
         const NodeRecord &rec = recs[i];
         switch (rec.kind) {
@@ -3002,10 +3274,18 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
             // Tag 1: the standalone overlap tasks, no solver reads the joints.
             if (rec.userTag != 1) launchSortArchetype(ex, ph->hPhys.jointArchetype, 1, s);
             // the search appends the step's pairs to empty lists: hull - hull, other and, with
-            // a hull past the staging caps, large (tickets are zero between launches)
+            // a hull past the staging caps, large; with worlds past 128 bodies also the list
+            // of those worlds (tickets are zero between launches)
             cudaMemsetAsync(ph->hPhys.hullPairs.counters, 0,
-                            (ph->largeHulls ? 3 : 2) * sizeof(PairListCounters), s);
+                            (large_worlds ? 4 : ph->largeHulls ? 3 : 2) * sizeof(PairListCounters), s);
             physFindCandidatesKernel<<<wgrid, wblock, 0, s>>>(d);
+            if (large_worlds) {
+                if (ph->largeSearchBlocks == 0) {
+                    *err = "large-world candidate search occupancy query failed";
+                    return false;
+                }
+                physFindCandidatesLargeKernel<<<ph->largeSearchBlocks, kLargeSearchThreads, 0, s>>>(d);
+            }
             break;
         case NodePhysSubstepBegin:
             physBodyKernel<PhaseIntegrate><<<bgrid, 256, 0, s>>>(d);

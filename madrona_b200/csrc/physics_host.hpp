@@ -8,6 +8,8 @@ namespace mb2 {
 
 // MADRONA_B200_MAX_HULL_SIZE (16 when unset), or false and why its value is invalid
 bool physicsMaxHullSize(int *size, std::string *err);
+// MADRONA_B200_MAX_BODIES_PER_WORLD (128 when unset), or false and why its value is invalid
+bool physicsMaxWorldBodies(int *bodies, std::string *err);
 bool physicsHostCreate(Executor *ex, std::string *err);
 bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *rc, std::string *err);
 void physicsHostDestroy(Executor *ex);

@@ -172,7 +172,12 @@ enum PrimClass : unsigned char {
     PrimLarge = 1,      // a hull within PhysicsState::maxHullSize vertices and faces
     PrimTooLarge = 2,   // a hull past it: the pair raises ErrPhysicsOverflow
 };
-constexpr int kMaxLevelBodies = 128;  // bodies per world tracked by the contact level scan
+constexpr int kMaxLevelBodies = 128;  // bodies per world tracked by the contact level scan in shared memory
+// MADRONA_B200_MAX_BODIES_PER_WORLD: BVH leaves (rigid bodies) a world may hold.  Worlds of
+// up to kMinWorldBodiesCap leaves take the warp-per-world candidate search and the shared
+// level table; larger ones, up to the knob, the block-per-world search and a global table.
+constexpr int kMinWorldBodiesCap = 128;
+constexpr int kMaxWorldBodiesCap = 4096;
 
 struct BodyArchetype {
     u32 archetype;
@@ -229,6 +234,16 @@ struct PhysicsState {
     // the step's pairs with a large or too large primitive, of every pair type: the third
     // work list, read by physNarrowphaseLargeKernel
     PairList largePairs;
+
+    // ---- worlds past 128 bodies (MADRONA_B200_MAX_BODIES_PER_WORLD > 128)
+    i32 maxWorldBodies;          // 128: none of the fields below is used
+    // the step's worlds with 128 < numTraversal <= maxWorldBodies, PairEntry { world,
+    // numTraversal }: appended by physFindCandidatesKernel, searched by
+    // physFindCandidatesLargeKernel (one block per world)
+    PairList largeWorlds;
+    // [numWorlds][maxWorldBodies] per-body contact levels of the worlds with more body
+    // slots than the shared table holds (orderContacts)
+    i32 *levelScratch;
 };
 
 }

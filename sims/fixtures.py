@@ -444,6 +444,27 @@ SIMS: Dict[str, SimDesc] = {
         objects=_triggers_objects,
         compile_flags=["-DTRIGGERS_WITH_SOLVER=1"],
     ),
+    # worlds of 20 to 1500 bodies whose sizes change every episode (or uniform_bodies for all),
+    # past the 128-body warp-per-world candidate search (tests/test_large_physics_worlds.py);
+    # layout 1 clusters the bodies into a tree deeper than the rebuild's stacks (GPU only)
+    "crowd": SimDesc(
+        name="crowd",
+        sources=[os.path.join(_ROOT, "crowd", "sim.cpp")],
+        num_exports=5,
+        num_taskgraphs=1,
+        inputs=[],
+        outputs=[Slot(0, "body_pos", "float32", (3,), dynamic=True),
+                 Slot(1, "body_rot", "float32", (4,), dynamic=True),
+                 Slot(2, "body_vel", "float32", (6,), dynamic=True),
+                 Slot(3, "body_entity", "int32", (2,), dynamic=True),
+                 Slot(4, "body_count", "int32", (1,))],
+        pack_config=lambda cfg: struct.pack("<QIIII", int(cfg.get("obj_mgr_ptr", 0)), int(cfg["episode_len"]),
+                                            int(cfg["uniform_bodies"]), int(cfg["layout"]), 0),
+        pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
+        oracle_extra=lambda cfg: [int(cfg.get("seed", 0)), int(cfg["episode_len"]), int(cfg["uniform_bodies"])],
+        defaults={"seed": 0, "episode_len": 40, "uniform_bodies": 0, "layout": 0},
+        objects=_hullpile_objects,
+    ),
     "gridworld": SimDesc(
         name="gridworld",
         sources=[os.path.join(_ROOT, "gridworld", "sim.cpp")],
