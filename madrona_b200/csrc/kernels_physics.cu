@@ -2301,7 +2301,7 @@ __device__ __forceinline__ BodyPair bodyPair(const BodyMass &m1, const BodyMass 
 // body has exactly one live copy during the solve and results do not depend on
 // kStagedBodies.  Slots count rows awaiting compaction too: room (33 bodies) fits,
 // arena's highest slots spill.  A block of 64 threads stages 32 * kPhysWarps /
-// kSolverLanes worlds: 13.6 KB of static shared memory at 16 lanes per world.
+// kPosSolverLanes worlds: 13.6 KB of static shared memory at 16 lanes per world.
 constexpr int kStagedBodies = 48;
 
 struct PosBody {                // x, q read / write
@@ -2512,12 +2512,18 @@ __device__ void solveJoint(EngineState &S, const PhysicsState &P, const ObjectMa
 // keep their sequential order.  Inside a level the members are compacted onto
 // the group's first lanes (ballot + find-nth-set).
 // Several worlds per warp multiply the worlds in flight per SM at no register
-// cost.  Measured on room at 8192 worlds (H100, staged position solve): 16 lanes
-// per world 1.515 ms/step (position solve 0.371, velocity solve 0.256 ms/step),
-// 8 lanes 1.537 (0.426, 0.225), parent code at 8 lanes 1.604 (0.496, 0.219).
-// 4 lanes does not fit: 16 staged worlds per block exceed 48 KB of static
-// shared memory.
-constexpr int kSolverLanes = 16;
+// cost.  Measured on room at 8192 worlds (H100, staged position solve, both solves
+// at 16 lanes): 16 lanes per world 1.515 ms/step (position solve 0.371, velocity
+// solve 0.256 ms/step), both at 8 lanes 1.537 (0.426, 0.225).  So each solve has its
+// own lane count.  The position solve keeps 16 lanes: a level's contacts spread over
+// more lanes, and 4 lanes does not fit (16 staged worlds per block exceed 48 KB of
+// static shared memory).  The velocity solve fits 8 blocks of 64 threads per SM
+// (121 registers at 16 lanes, 128 at 8): 32 worlds per SM at 16 lanes, 64 at 8.
+// velocitySolveLanes keeps 16 lanes while the worlds fit one wave of that (arena:
+// 4096 worlds on 132 SMs) and takes 8 past it (room: 8192 worlds in one wave
+// instead of two).
+constexpr int kPosSolverLanes = 16;
+constexpr int kVelSolveBlocksPerSM = 8;
 
 template <int LPW, typename Fn>
 __device__ __forceinline__ void sweepContactLevels(const Contact *contacts, const i32 *order, const i32 n,
@@ -2565,9 +2571,9 @@ __device__ void phaseSolvePositions(EngineState &S, const PhysicsState &P, const
                                     const int lane, PosBody *stage)
 {
     const ObjectManager &objs = worldObjects(S, P, w);
-    const int sub = lane & (kSolverLanes - 1);
+    const int sub = lane & (kPosSolverLanes - 1);
     if (valid) {
-        forEachStagedBody<kSolverLanes>(S, P, w, sub, [&](i32 slot, u32 arch, i32 row) {
+        forEachStagedBody<kPosSolverLanes>(S, P, w, sub, [&](i32 slot, u32 arch, i32 row) {
             stage[slot] = globalPosBody(S, P, objs, arch, row);
         });
     }
@@ -2577,7 +2583,7 @@ __device__ void phaseSolvePositions(EngineState &S, const PhysicsState &P, const
     const i32 *order = P.contactOrder + (size_t)w * P.maxContactsPerWorld;
     const i32 n = valid ? P.contactCounts[w] : 0;
     const i32 levels = valid ? P.contactMaxLevel[w] : 0;
-    sweepContactLevels<kSolverLanes>(contacts, order, n, levels, lane, [&](i32 i) {
+    sweepContactLevels<kPosSolverLanes>(contacts, order, n, levels, lane, [&](i32 i) {
         solveContactPosition(S, P, objs, stage, contacts[i]);
     });
 
@@ -2595,7 +2601,7 @@ __device__ void phaseSolvePositions(EngineState &S, const PhysicsState &P, const
     __syncwarp();
 
     if (valid) {
-        forEachStagedBody<kSolverLanes>(S, P, w, sub, [&](i32 slot, u32 arch, i32 row) {
+        forEachStagedBody<kPosSolverLanes>(S, P, w, sub, [&](i32 slot, u32 arch, i32 row) {
             cachedCol<Vector3>(arch, PCPosition, row) = stage[slot].x;
             cachedCol<Quat>(arch, PCRotation, row) = stage[slot].q;
         });
@@ -2706,6 +2712,7 @@ __device__ void solveContactVelocity(EngineState &S, const PhysicsState &P, cons
 
 // Not staged: with the velocity sweep's shorter load chains, copying every body
 // in and out cost more than the sweep saved (DESIGN.md 3.2).
+template <int LPW>
 __device__ void phaseSolveVelocities(EngineState &S, const PhysicsState &P, const i32 w, const bool valid,
                                      const int lane)
 {
@@ -2715,7 +2722,7 @@ __device__ void phaseSolveVelocities(EngineState &S, const PhysicsState &P, cons
     const i32 *order = P.contactOrder + (size_t)w * P.maxContactsPerWorld;
     const i32 n = valid ? P.contactCounts[w] : 0;
     const i32 levels = valid ? P.contactMaxLevel[w] : 0;
-    sweepContactLevels<kSolverLanes>(contacts, order, n, levels, lane, [&](i32 i) {
+    sweepContactLevels<LPW>(contacts, order, n, levels, lane, [&](i32 i) {
         solveContactVelocity(S, P, objs, contacts[i], params.h, params.restitutionThreshold);
     });
 }
@@ -2724,8 +2731,8 @@ __device__ void phaseSolveVelocities(EngineState &S, const PhysicsState &P, cons
 // Launchers.  Row-parallel phases (leaf update + refit, integrate, velocity
 // update) are grid-stride kernels over all rows of every body archetype; the
 // candidate search gives each world a warp, the solves give each world
-// kSolverLanes lanes (and the position solve a shared-memory copy of its
-// bodies, kStagedBodies).
+// kPosSolverLanes / velocitySolveLanes lanes (and the position solve a shared-memory
+// copy of its bodies, kStagedBodies).
 // (A single fused warp-per-world kernel for the whole step would spread its warps
 // over every phase of a large instruction footprint, and the light phases would
 // inherit the narrowphase's register count and occupancy.)
@@ -2775,7 +2782,8 @@ physRebuildKernel(EngineState *Sp)
 }
 
 // The per-world kernels run kPhysWarps warps per block: one world per warp in the
-// candidate search, 32 / kSolverLanes worlds per warp in the solves.
+// candidate search, 32 / kPosSolverLanes resp. 32 / velocitySolveLanes worlds per
+// warp in the solves.
 constexpr int kPhysWorldThreads = 32 * kPhysWarps;
 
 __global__ void __launch_bounds__(kPhysWorldThreads, 8)
@@ -2827,20 +2835,30 @@ physFindCandidatesLargeKernel(EngineState *Sp)
     });
 }
 
-// kSolverLanes lanes per world.  The lanes of a warp past the last world idle along
-// on the last world (valid = false); returns false when the whole warp is past it.
+// LPW lanes per world.  The lanes of a warp past the last world idle along on the
+// last world (valid = false); returns false when the whole warp is past it.
+template <int LPW>
 __device__ __forceinline__ bool solverWorld(const EngineState &S, i32 &w, bool &valid)
 {
-    const i32 first_w = (i32)((blockIdx.x * blockDim.x + (threadIdx.x & ~31u)) / kSolverLanes);
+    const i32 first_w = (i32)((blockIdx.x * blockDim.x + (threadIdx.x & ~31u)) / LPW);
     if (first_w >= (i32)S.numWorlds) return false;
-    const i32 my_w = (i32)((blockIdx.x * blockDim.x + threadIdx.x) / kSolverLanes);
+    const i32 my_w = (i32)((blockIdx.x * blockDim.x + threadIdx.x) / LPW);
     valid = my_w < (i32)S.numWorlds;
     w = valid ? my_w : (i32)S.numWorlds - 1;
     return true;
 }
 
-// physicsHostAfterRegistry sets this kernel's carveout to the maximum shared memory
-// for its body stage.
+// physicsHostAfterRegistry sets this kernel's carveout to kPosSolveCarveoutPercent: 132 KB of
+// the SM's 228 KB maximum, the smallest H100 configuration that holds its 8 blocks (static
+// stage + the 1 KB the driver reserves per block).  The other 124 KB of the SM's 256 KB stay
+// L1, which keeps the contacts and the PreSolvePositional / SubstepPrevState rows that every
+// level of a world re-reads.  Measured on room at 8192 worlds (H100 80GB HBM3, 700 W): the
+// node took 0.342 ms/step with the maximum carveout, 0.303 at 164 KB, 0.289 at 132 KB.
+constexpr int kPosSolveCarveoutPercent = 58;
+static_assert(8 * (sizeof(ColCache) + (kPhysWorldThreads / kPosSolverLanes) *
+                   (sizeof(i32) * kMaxLevelBodies + sizeof(PosBody) * kStagedBodies) + 1024) <= 132 * 1024,
+              "8 position-solve blocks no longer fit the 132 KB shared-memory configuration");
+
 __global__ void __launch_bounds__(kPhysWorldThreads, 8)
 physSolvePositionsKernel(EngineState *Sp)
 {
@@ -2850,15 +2868,16 @@ physSolvePositionsKernel(EngineState *Sp)
     const int lane = threadIdx.x & 31;
     i32 w;
     bool valid;
-    if (!solverWorld(S, w, valid)) return;
-    constexpr int kWorldsPerBlock = kPhysWorldThreads / kSolverLanes;
+    if (!solverWorld<kPosSolverLanes>(S, w, valid)) return;
+    constexpr int kWorldsPerBlock = kPhysWorldThreads / kPosSolverLanes;
     __shared__ i32 last_level[kWorldsPerBlock][kMaxLevelBodies];
     __shared__ PosBody pos_stage[kWorldsPerBlock][kStagedBodies];
-    orderContacts<kSolverLanes>(S, P, w, valid, lane, last_level[threadIdx.x / kSolverLanes]);
-    phaseSolvePositions(S, P, w, valid, lane, pos_stage[threadIdx.x / kSolverLanes]);
+    orderContacts<kPosSolverLanes>(S, P, w, valid, lane, last_level[threadIdx.x / kPosSolverLanes]);
+    phaseSolvePositions(S, P, w, valid, lane, pos_stage[threadIdx.x / kPosSolverLanes]);
 }
 
-__global__ void __launch_bounds__(kPhysWorldThreads, 8)
+template <int LPW>
+__global__ void __launch_bounds__(kPhysWorldThreads, kVelSolveBlocksPerSM)
 physSolveVelocitiesKernel(EngineState *Sp)
 {
     EngineState &S = *Sp;
@@ -2867,8 +2886,8 @@ physSolveVelocitiesKernel(EngineState *Sp)
     const int lane = threadIdx.x & 31;
     i32 w;
     bool valid;
-    if (!solverWorld(S, w, valid)) return;
-    phaseSolveVelocities(S, P, w, valid, lane);
+    if (!solverWorld<LPW>(S, w, valid)) return;
+    phaseSolveVelocities<LPW>(S, P, w, valid, lane);
 }
 
 // =============================================================================================
@@ -3133,9 +3152,9 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::stri
         }
     }
     cudaMemcpy(ph->dPhys, &P, sizeof(PhysicsState), cudaMemcpyHostToDevice);
-    // the position solve's body stage: prefer shared memory over L1 (measured with this setting)
+    // the position solve's body stage, and L1 for the rest (see kPosSolveCarveoutPercent)
     if (cudaFuncSetAttribute(physSolvePositionsKernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                             (int)cudaSharedmemCarveoutMaxShared) != cudaSuccess) {
+                             kPosSolveCarveoutPercent) != cudaSuccess) {
         *err = "setting the position solve's shared-memory carveout failed";
         return false;
     }
@@ -3238,6 +3257,16 @@ static dim3 bodyGrid(Executor *ex)
     return dim3((unsigned)std::max(blocks, 1), std::max(P.numBodyArchetypes, 1u));
 }
 
+// Lanes per world of the velocity solve: 16 while the worlds fit one wave of the
+// 16-lane kernel (kVelSolveBlocksPerSM blocks of 4 worlds per SM), else 8.  Fewer
+// lanes per world spread a level's contacts over fewer lanes but double the worlds
+// resident at once.
+static unsigned velocitySolveLanes(const Executor *ex, unsigned W)
+{
+    const unsigned wide_worlds = (unsigned)ex->numSMs * kVelSolveBlocksPerSM * (kPhysWorldThreads / 16);
+    return W <= wide_worlds ? 16u : 8u;
+}
+
 bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, cudaStream_t s,
                          std::string *err)
 {
@@ -3254,8 +3283,9 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
     const unsigned W = ex->hState->numWorlds;
     const unsigned wgrid = (W + kPhysWarps - 1) / kPhysWarps;
     const unsigned wblock = kPhysWorldThreads;
-    const unsigned worlds_per_block = wblock / kSolverLanes;
-    const unsigned sgrid = (W + worlds_per_block - 1) / worlds_per_block;
+    const unsigned pos_grid = (W + wblock / kPosSolverLanes - 1) / (wblock / kPosSolverLanes);
+    const unsigned vel_lanes = velocitySolveLanes(ex, W);
+    const unsigned vel_grid = (W + wblock / vel_lanes - 1) / (wblock / vel_lanes);
     const dim3 bgrid = bodyGrid(ex);
     const bool large_worlds = ph->hPhys.maxWorldBodies > kMinWorldBodiesCap;
     for (uint32_t i = 0; i < count; i++) {
@@ -3307,7 +3337,7 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
             }
             break;
         case NodePhysSolvePositions:
-            physSolvePositionsKernel<<<sgrid, wblock, 0, s>>>(d);
+            physSolvePositionsKernel<<<pos_grid, wblock, 0, s>>>(d);
             break;
         case NodePhysTGSVelocities:
             physBodyKernel<PhaseTGSVelocities><<<bgrid, 256, 0, s>>>(d);
@@ -3319,7 +3349,8 @@ bool physicsEnqueueNodes(Executor *ex, const NodeRecord *recs, uint32_t count, c
             physBodyKernel<PhaseSetVelocities><<<bgrid, 256, 0, s>>>(d);
             break;
         case NodePhysSolveVelocities:
-            physSolveVelocitiesKernel<<<sgrid, wblock, 0, s>>>(d);
+            if (vel_lanes == 16) physSolveVelocitiesKernel<16><<<vel_grid, wblock, 0, s>>>(d);
+            else physSolveVelocitiesKernel<8><<<vel_grid, wblock, 0, s>>>(d);
             break;
         case NodePhysEmitOverlaps: {
             const EngineState &S = *ex->hState;
