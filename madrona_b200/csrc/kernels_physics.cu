@@ -507,15 +507,26 @@ __device__ __forceinline__ void rowRefit(const EngineState &S, const PhysicsStat
 }
 
 // A body takes part in contact ordering unless writing it back is a no-op:
-// static (inverse mass / inertia forced to 0, so x is unchanged) AND its
-// rotation is a bitwise fixpoint of normalize() (so q is unchanged).  Decided
-// once per step by the candidate search (a fixpoint stays one: the solvers
-// write back normalize(q) == q; treating a body that BECAME a fixpoint during
-// the step as still mutable only adds ordering edges, never removes one).
+// static (inverse mass / inertia forced to 0, so the solves add exactly +-0 to
+// x and q) AND its rotation is a bitwise fixpoint of normalize() AND no
+// component of x or q is -0 (-0 + (+0) == +0: two writers of one level would
+// store -0 and +0, where the sequential sweep ends at +0).  Decided once per
+// step by the candidate search (a fixpoint stays one: the solvers write back
+// normalize(q) == q; treating a body that BECAME a fixpoint during the step as
+// still mutable only adds ordering edges, never removes one).
 __device__ __forceinline__ bool rotationIsNormalizeFixpoint(Quat q)
 {
     const Quat n = q.normalize();
     return n.w == q.w && n.x == q.x && n.y == q.y && n.z == q.z;
+}
+
+__device__ __forceinline__ bool isNegativeZero(float f) { return __float_as_uint(f) == 0x80000000u; }
+
+__device__ __forceinline__ bool writeBackIsNoOp(Vector3 x, Quat q)
+{
+    if (isNegativeZero(x.x) || isNegativeZero(x.y) || isNegativeZero(x.z)) return false;
+    if (isNegativeZero(q.w) || isNegativeZero(q.x) || isNegativeZero(q.y) || isNegativeZero(q.z)) return false;
+    return rotationIsNormalizeFixpoint(q);
 }
 
 constexpr u32 kUnknownSlot = 0x7fffu;
@@ -580,7 +591,10 @@ __device__ __forceinline__ u32 bodySlotInfo(const EngineState &S, const PhysicsS
 {
     const i32 slot = worldBodySlot(S, P, w, arch, row);
     bool is_mutable = true;
-    if (is_static) is_mutable = !rotationIsNormalizeFixpoint(cachedCol<Quat>(arch, PCRotation, row));
+    if (is_static) {
+        is_mutable = !writeBackIsNoOp(cachedCol<Vector3>(arch, PCPosition, row),
+                                      cachedCol<Quat>(arch, PCRotation, row));
+    }
     const u32 s15 = (slot < 0 || slot >= (i32)kUnknownSlot) ? kUnknownSlot : (u32)slot;
     return (s15 << 1) | (is_mutable ? 1u : 0u);
 }
