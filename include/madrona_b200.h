@@ -84,8 +84,13 @@ typedef struct mb2_material_view {
  * zero-initialises the struct): a render_resolution square.  Set together; a
  * nonzero render_resolution must then equal both.  The vertical field of view
  * spans the rows, the horizontal one is widened by width / height.
- * render_width * render_height * 4 must fit in 32 bits.  mb2_executor_create
- * returns NULL and mb2_last_error() says why when any of this does not hold. */
+ * render_width * render_height * 4 must fit in 32 bits.  segmentation = 1 (not
+ * in the reference) gives every view one more output, row-major
+ * [render_height][render_width] int32: the Entity id (without its generation) of
+ * the renderable that the pixel's primary ray hits first, -1 where the ray hits
+ * nothing, so -1 exactly where the depth is 0; 0 (zero-initialised) leaves it out.
+ * mb2_executor_create returns NULL and mb2_last_error() says why when any of this
+ * does not hold (segmentation is 0 or 1). */
 typedef struct mb2_render_config {
     uint32_t render_mode;          /* 0 RGBD, 1 Depth */
     mb2_mesh_bvh_view geo_bvh_data;
@@ -95,6 +100,7 @@ typedef struct mb2_render_config {
     float far_plane;
     uint32_t render_width;         /* columns per view, or 0 */
     uint32_t render_height;        /* rows per view, or 0 */
+    uint32_t segmentation;         /* 1: per-pixel entity ids, 0: none */
 } mb2_render_config;
 
 /* Triangle mesh -> BLAS.  Role of MeshBVHBuilder (src/common/mesh_bvh_builder.cpp,

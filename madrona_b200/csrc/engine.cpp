@@ -361,10 +361,10 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
         return false;
     }
     if (rc) {
-        // the image size is checked before any CUDA call or allocation
-        uint32_t width, height;
+        // the image size and the segmentation flag are checked before any CUDA call or allocation
+        uint32_t width, height, segmentation;
         std::string err;
-        if (!renderImageSize(rc, &width, &height, &err)) {
+        if (!renderImageSize(rc, &width, &height, &err) || !renderSegmentation(rc, &segmentation, &err)) {
             setError(err);
             return false;
         }

@@ -10,7 +10,8 @@
 //   renderScanInstancesKernel    world offsets into the compact instance list, list of the
 //                                worlds above kWarpTLASInstances
 //   renderGatherInstancesKernel  every world's renderable instances -> InstanceData +
-//                                world box (mesh root box under TRS), at the world's offset
+//                                world box (mesh root box under TRS) + entity id, at the
+//                                world's offset
 //   renderLightKernels           carriers refresh their LightDesc, lights gathered per world
 //   renderGatherViewsKernel      PerspectiveCameraData per view
 //   renderBuildTLASKernel        worlds of <= kWarpTLASInstances: ONE WARP PER WORLD, all in
@@ -27,7 +28,7 @@
 // (reference-format MeshBVH: quantised 4-wide nodes over de-indexed triangles)
 // -> watertight ray / triangle test; materials (override colour / material
 // table, material textures sampled at the final hit's uv), lights with shadow
-// rays, RGBA8 + f32 depth.
+// rays, RGBA8 + f32 depth (+ the hit entity's id when the config asks for segmentation).
 //
 // Image formation follows the reference's CUDA ray tracer
 // (src/mw/device/bvh_raycast.cpp): ray generation :58-88, object-space ray and
@@ -254,6 +255,8 @@ renderGatherInstancesKernel(EngineState *Sp)
                     }
                     inst.aabbMin[0] = box.pMin.x; inst.aabbMin[1] = box.pMin.y; inst.aabbMin[2] = box.pMin.z;
                     inst.aabbMax[0] = box.pMax.x; inst.aabbMax[1] = box.pMax.y; inst.aabbMax[2] = box.pMax.z;
+                    // column 0 is the row's Entity {gen, id}: the id is the high word
+                    inst.entityID = (i32)(u32)(((const u64 *)t.columns[0])[row] >> 32);
                     out[at] = inst;
                 }
             }
@@ -1431,6 +1434,11 @@ renderRaycastKernel(EngineState *Sp)
             const size_t off = (size_t)view.outputRow * bytes_per_view + 4 * pix;
             float *depth_out = (float *)((char *)out_tbl.columns[R.depthCol] + off);
             *depth_out = hit ? first.t : 0.f;
+            if (R.segmentation) {
+                // the same closest hit as the depth: -1 exactly where the depth is 0
+                i32 *seg_out = (i32 *)((char *)out_tbl.columns[R.segCol] + off);
+                *seg_out = hit ? instances[first.instance].entityID : -1;
+            }
             if (R.hitIDs) {
                 i32 *ids = R.hitIDs + ((size_t)view.outputRow * pixels_per_view + pix) * 2;
                 ids[0] = hit ? first.instance : -1;
@@ -1574,10 +1582,21 @@ bool renderImageSize(const mb2_render_config *rc, u32 *width, u32 *height, std::
     return true;
 }
 
+// Whether a render config asks for the segmentation output (0 off, 1 on; else invalid).
+bool renderSegmentation(const mb2_render_config *rc, u32 *on, std::string *err)
+{
+    if (rc->segmentation > 1) {
+        *err = "segmentation = " + std::to_string(rc->segmentation) + " is not 0 (off) or 1 (on)";
+        return false;
+    }
+    *on = rc->segmentation;
+    return true;
+}
+
 bool renderHostCreate(Executor *ex, const mb2_render_config *rc, std::string *err)
 {
-    u32 width = 0, height = 0;
-    if (rc && !renderImageSize(rc, &width, &height, err)) return false;
+    u32 width = 0, height = 0, segmentation = 0;
+    if (rc && (!renderImageSize(rc, &width, &height, err) || !renderSegmentation(rc, &segmentation, err))) return false;
     RenderHost *rh = new RenderHost();
     ex->render = rh;
     memset(&rh->hRender, 0, sizeof(RenderState));
@@ -1597,6 +1616,7 @@ bool renderHostCreate(Executor *ex, const mb2_render_config *rc, std::string *er
         R.width = width;
         R.height = height;
         R.rgbd = rc->render_mode == 0 ? 1u : 0u;
+        R.segmentation = segmentation;
         R.nearPlane = rc->near_plane;
         R.farPlane = rc->far_plane;
         // device pointers, adopted as they are (the reference frees them in its
@@ -1665,6 +1685,7 @@ bool renderHostAfterRegistry(Executor *ex, std::string *err)
     }
     R.rgbCol = col(R.outputArchetype, R.cidRGB);
     R.depthCol = col(R.outputArchetype, R.cidDepth);
+    R.segCol = col(R.outputArchetype, R.cidSegmentation);
     R.lightCol = col(R.lightArchetype, R.cidLightDesc);
     // the output table may grow (during world construction or between steps): the view
     // list covers every row it can ever have, so no view is left unrendered
@@ -1875,13 +1896,14 @@ LaunchGraph *physicsBuildRenderGraph(Executor *ex, std::string *err)
     return g;
 }
 
-// algorithmic bytes of one frame (SURVEY.md 8d): W x H x 4 B depth (+ 4 B RGBA8) per view
+// algorithmic bytes of one frame (SURVEY.md 8d): W x H x 4 B depth (+ 4 B RGBA8)
+// (+ 4 B segmentation) per view
 uint64_t renderBytesPerFrame(Executor *ex, int64_t num_views)
 {
     RenderHost *rh = ex->render;
     if (!rh || !rh->active) return 0;
     const RenderState &R = rh->hRender;
-    return (uint64_t)num_views * R.width * R.height * (R.rgbd ? 8ull : 4ull);
+    return (uint64_t)num_views * R.width * R.height * (4ull + (R.rgbd ? 4ull : 0ull) + (R.segmentation ? 4ull : 0ull));
 }
 
 }

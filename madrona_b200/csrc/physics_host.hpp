@@ -21,6 +21,8 @@ LaunchGraph *physicsBuildRenderGraph(Executor *ex, std::string *err);
 // batch ray-cast renderer (kernels_render.cu)
 // the image size of a render config, or false and why the config is invalid
 bool renderImageSize(const mb2_render_config *rc, uint32_t *width, uint32_t *height, std::string *err);
+// whether a render config asks for the segmentation output, or false and why it is invalid
+bool renderSegmentation(const mb2_render_config *rc, uint32_t *on, std::string *err);
 bool renderHostCreate(Executor *ex, const mb2_render_config *rc, std::string *err);
 bool renderHostAfterRegistry(Executor *ex, std::string *err);
 void renderHostDestroy(Executor *ex);

@@ -12,7 +12,7 @@ struct RVec3 { float x, y, z; };
 struct RQuat { float w, x, y, z; };
 
 // == render::InstanceData (include/madrona/render/ecs.hpp:49-63) + the instance's
-// world box (TLBVHNode in the reference)
+// world box (TLBVHNode in the reference) + the id of its entity (segmentation output)
 struct RenderInstance {
     RVec3 position;
     RQuat rotation;
@@ -22,7 +22,9 @@ struct RenderInstance {
     u32 color;            // 0xRRGGBB (ColorOverride)
     float aabbMin[3];
     float aabbMax[3];
+    i32 entityID;         // Entity::id of the renderable row (its gen is not kept)
 };
+static_assert(sizeof(RenderInstance) == 80, "RenderInstance layout");
 
 // == render::LightDesc (include/madrona/render/ecs.hpp:65-89), unpacked
 struct RenderLight {
@@ -84,6 +86,7 @@ struct RenderState {
     u32 numMeshes;
     const RenderMaterial *materials;   // device, == materialData.materials (may be null)
     u32 debugHits;                  // MADRONA_B200_RENDER_DEBUG: keep (instance, triangle) per pixel
+    u32 segmentation;               // 1: each view also gets an i32 entity id per pixel
 
     // ---- written by the device-side RenderingSystem::registerTypes
     u32 registered;
@@ -91,14 +94,14 @@ struct RenderState {
     u32 lightArchetype, cidLightDesc;
     u32 cidPosition, cidRotation, cidScale, cidObjectID;
     u32 outputArchetype;   // RaycastOutputArchetype
-    u32 cidRGB, cidDepth;
+    u32 cidRGB, cidDepth, cidSegmentation;
 
     // ---- filled by the host after registerTypes
     u32 numRenderArchetypes;
     RenderArchetype renderables[kMaxRenderArchetypes];
     u32 numViewArchetypes;
     ViewArchetype viewers[kMaxRenderArchetypes];
-    i32 rgbCol, depthCol;
+    i32 rgbCol, depthCol, segCol;
 
     // Instances are one world-major list: world w's, in gather order, start at
     // instanceOffsets[w] (exclusive scan of instanceCounts).  The list, the TLAS nodes and

@@ -72,10 +72,14 @@ struct RenderOutputBuffer {
 
 struct RGBOutputBuffer : RenderOutputBuffer {};
 struct DepthOutputBuffer : RenderOutputBuffer {};
+// Not in the reference: height x width i32 per view, the Entity::id of the renderable each
+// pixel's primary ray hits first, -1 where it hits nothing (mb2_render_config::segmentation)
+struct SegmentationOutputBuffer : RenderOutputBuffer {};
 
 struct RaycastOutputArchetype : public Archetype<
     RGBOutputBuffer,
-    DepthOutputBuffer
+    DepthOutputBuffer,
+    SegmentationOutputBuffer
 > {};
 
 struct RenderECSBridge;
@@ -106,6 +110,8 @@ inline void registerTypes(ECSRegistry &registry, const RenderECSBridge *)
     if (bytes == 0) bytes = 4;
     registry.registerComponent<RGBOutputBuffer>(bytes);
     registry.registerComponent<DepthOutputBuffer>(bytes);
+    // a view row carries 4 bytes of it when segmentation is off
+    registry.registerComponent<SegmentationOutputBuffer>(R.segmentation ? bytes : 4u);
     registry.registerArchetype<RaycastOutputArchetype>();
     registry.registerArchetype<LightArchetype>();
 
@@ -122,6 +128,7 @@ inline void registerTypes(ECSRegistry &registry, const RenderECSBridge *)
     R.outputArchetype = TypeTracker::typeID<RaycastOutputArchetype>();
     R.cidRGB = TypeTracker::typeID<RGBOutputBuffer>();
     R.cidDepth = TypeTracker::typeID<DepthOutputBuffer>();
+    R.cidSegmentation = TypeTracker::typeID<SegmentationOutputBuffer>();
     R.registered = 1;
 }
 

@@ -117,7 +117,7 @@ class _MaterialViewC(ctypes.Structure):      # == render::MaterialData
     ]
 
 
-class _RenderConfigC(ctypes.Structure):      # == madrona::CudaBatchRenderConfig + image size
+class _RenderConfigC(ctypes.Structure):      # == madrona::CudaBatchRenderConfig + image size + outputs
     _fields_ = [
         ("render_mode", ctypes.c_uint32),
         ("geo_bvh_data", _MeshBVHViewC),
@@ -128,6 +128,8 @@ class _RenderConfigC(ctypes.Structure):      # == madrona::CudaBatchRenderConfig
         # non-square images: both nonzero, render_resolution 0 (or equal to both)
         ("render_width", ctypes.c_uint32),
         ("render_height", ctypes.c_uint32),
+        # 1: per view one more output, int32 [height][width]: the hit entity's id, -1 on a miss
+        ("segmentation", ctypes.c_uint32),
     ]
 
 
@@ -519,7 +521,8 @@ class MWCudaExecutor:
         """(tlas_nodes u8 [N, 60], tlas_counts [W], instances u8 [N, 76], instance_counts [W],
         instance_offsets [W]) of the last render-prepare (test hook).  Compact layouts: world w's
         instances and TLAS nodes (node 0 = root) start at instance_offsets[w]; N = visible
-        instances of all worlds."""
+        instances of all worlds.  An instance is the first 76 bytes of its 80-byte record:
+        InstanceData and world box, without the entity id that follows."""
         import torch
         stride = ctypes.c_int64(0)
 
@@ -533,7 +536,7 @@ class MWCudaExecutor:
         ncount, icount, offsets = fetch(2, (W,), "<i4"), fetch(4, (W,), "<i4"), fetch(5, (W,), "<i4")
         total = int(offsets[-1] + icount[-1])
         nodes = fetch(1, (max(total, 1), 60), "|u1")[:total]
-        inst = fetch(3, (max(total, 1), 76), "|u1")[:total]
+        inst = fetch(3, (max(total, 1), 80), "|u1")[:total, :76]
         return nodes, ncount, inst, icount, offsets
 
     def peerGather(self, slots, shapes, dtypes, world_size: int, rank: int):

@@ -151,6 +151,15 @@ struct RenderImageSize {
     uint32_t height;
 };
 
+// Outputs beyond RGB and depth for the MWCudaExecutor constructor overload that takes them.
+// segmentation: every view also gets a row-major [height][width] int32 image, the Entity id
+// (without its generation) of the renderable each pixel's primary ray hits first, -1 where
+// it hits nothing.  Exported like the other outputs, through
+// exportColumn<render::RaycastOutputArchetype, render::SegmentationOutputBuffer>.
+struct RenderOutputs {
+    bool segmentation;
+};
+
 // A device-memory snapshot of an executor's simulation state (include/madrona_b200.h),
 // made by MWCudaExecutor::snapshot().  save() / restore() are one kernel launch each on
 // `strm` (by default the executor's stream) and never synchronize the host; stepping after
@@ -238,7 +247,8 @@ public:
                    const Optional<CudaBatchRenderConfig> &render_cfg =
                        Optional<CudaBatchRenderConfig>::none())
     {
-        create(state_cfg, compile_cfg, cu_ctx, render_cfg, ::madrona_b200::RenderImageSize { 0, 0 });
+        create(state_cfg, compile_cfg, cu_ctx, render_cfg, ::madrona_b200::RenderImageSize { 0, 0 },
+               ::madrona_b200::RenderOutputs { false });
     }
 
     // Not in the reference: the batch renderer's images are image_size.width columns by
@@ -247,7 +257,17 @@ public:
                    CUcontext cu_ctx, const Optional<CudaBatchRenderConfig> &render_cfg,
                    const ::madrona_b200::RenderImageSize &image_size)
     {
-        create(state_cfg, compile_cfg, cu_ctx, render_cfg, image_size);
+        create(state_cfg, compile_cfg, cu_ctx, render_cfg, image_size, ::madrona_b200::RenderOutputs { false });
+    }
+
+    // Not in the reference: the image size as above (RenderImageSize { 0, 0 }: the
+    // renderResolution square) and the extra outputs every view gets.
+    MWCudaExecutor(const StateConfig &state_cfg, const CompileConfig &compile_cfg,
+                   CUcontext cu_ctx, const Optional<CudaBatchRenderConfig> &render_cfg,
+                   const ::madrona_b200::RenderImageSize &image_size,
+                   const ::madrona_b200::RenderOutputs &outputs)
+    {
+        create(state_cfg, compile_cfg, cu_ctx, render_cfg, image_size, outputs);
     }
 
     MWCudaExecutor(MWCudaExecutor &&o) : h_(o.h_) { o.h_ = nullptr; }
@@ -319,7 +339,8 @@ public:
 private:
     void create(const StateConfig &state_cfg, const CompileConfig &compile_cfg, CUcontext cu_ctx,
                 const Optional<CudaBatchRenderConfig> &render_cfg,
-                const ::madrona_b200::RenderImageSize &image_size)
+                const ::madrona_b200::RenderImageSize &image_size,
+                const ::madrona_b200::RenderOutputs &outputs)
     {
         mb2_state_config sc {
             state_cfg.worldInitPtr, state_cfg.numWorldInitBytes,
@@ -346,6 +367,7 @@ private:
             rc.far_plane = render_cfg->farPlane;
             rc.render_width = image_size.width;
             rc.render_height = image_size.height;
+            rc.segmentation = outputs.segmentation ? 1u : 0u;
         }
         int gpu_id = mb2_device_of_context((void *)cu_ctx);
         h_ = mb2_executor_create(&sc, &cc, gpu_id, render_cfg.has_value() ? &rc : nullptr);

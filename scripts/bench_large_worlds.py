@@ -71,7 +71,7 @@ def main():
     for props in [int(p) for p in args.props.split(",")]:
         visible = props - (props - 1) // 17
         prepare_ms, step_ms, render_ms = _measure(args.worlds, props, args.res, args.warmup, args.iters, args.reps)
-        # the TLAS build reads each instance record (76 B) and writes at most one 60 B node
+        # the TLAS build reads each instance record (80 B) and writes at most one 60 B node
         # per instance; the sort and tree passes touch 8 B keys and 52 B scratch entries
         print(json.dumps({
             "card": card, "power_limit": power, "worlds": args.worlds, "resolution": args.res,

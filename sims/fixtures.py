@@ -145,10 +145,16 @@ def _image_size(cfg, default_res):
     return {"resolution": int(cfg.get("resolution", default_res))}
 
 
+def _render_options(cfg, default_res):
+    """Keyword arguments for the render_assets builders: the image size, and `segmentation`
+    (per-pixel hit entity ids, off unless the fixture config sets it)."""
+    return dict(_image_size(cfg, default_res), segmentation=bool(cfg.get("segmentation", False)))
+
+
 def _room_render_cfg(cfg):
     from .render_assets import make_render_config
     return make_render_config(rgbd=bool(cfg.get("rgbd", False)), gpu_id=int(cfg.get("_gpu_id", 0)),
-                              **_image_size(cfg, 64))
+                              **_render_options(cfg, 64))
 
 
 SIMS: Dict[str, SimDesc] = {
@@ -266,7 +272,7 @@ SIMS: Dict[str, SimDesc] = {
     "room_render": SimDesc(
         name="room_render",
         sources=[os.path.join(_ROOT, "room", "sim.cpp")],
-        num_exports=17,
+        num_exports=19,
         num_taskgraphs=1,
         inputs=[Slot(0, "reset", "int32", (1,)), Slot(1, "action", "int32", (2, 3))],
         outputs=[Slot(2, "reward", "float32", (2,)), Slot(3, "done", "int32", (2,)),
@@ -324,11 +330,12 @@ SIMS: Dict[str, SimDesc] = {
     "hullpile_big": _hullpile_desc("hullpile_big", 20, objects=_hullpile_big_objects),
     "hullpile_big_many": _hullpile_desc("hullpile_big_many", 60, ["-DHULLPILE_MANY=1"],
                                         objects=_hullpile_big_objects),
-    # GPU only: batch ray caster with a real TLAS / BLAS, materials, lights (tests/test_render_bvh.py)
+    # GPU only: batch ray caster with a real TLAS / BLAS, materials, lights (tests/test_render_bvh.py);
+    # -DGALLERY_ENTITY_EXPORTS=1 adds the props' entities and the segmentation output (slots 10, 11)
     "gallery": SimDesc(
         name="gallery",
         sources=[os.path.join(_ROOT, "gallery", "sim.cpp")],
-        num_exports=10,
+        num_exports=12,
         num_taskgraphs=1,
         inputs=[],
         outputs=[],
@@ -336,15 +343,16 @@ SIMS: Dict[str, SimDesc] = {
         pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
         oracle_extra=lambda cfg: [],
         defaults={"num_props": 100, "seed": 0, "resolution": 40, "rgbd": True},
+        compile_flags=["-DGALLERY_ENTITY_EXPORTS=1"],
         render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_render_config(
-            rgbd=bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)), **_image_size(cfg, 40)),
+            rgbd=bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)), **_render_options(cfg, 40)),
     ),
     # GPU only: the gallery built with -DGALLERY_PER_WORLD=1: props[w] props in world w (every
     # 17th hidden, as in the gallery), layouts[w] 0 scattered / 1 clustered (deep Morton tree)
     "gallery_sized": SimDesc(
         name="gallery_sized",
         sources=[os.path.join(_ROOT, "gallery", "sim.cpp")],
-        num_exports=10,
+        num_exports=12,
         num_taskgraphs=1,
         inputs=[],
         outputs=[],
@@ -353,16 +361,16 @@ SIMS: Dict[str, SimDesc] = {
                                              int(cfg["layouts"][w]) if cfg.get("layouts") else 0),
         oracle_extra=lambda cfg: [],
         defaults={"props": [100], "layouts": None, "seed": 0, "resolution": 40, "rgbd": True},
-        compile_flags=["-DGALLERY_PER_WORLD=1"],
+        compile_flags=["-DGALLERY_PER_WORLD=1", "-DGALLERY_ENTITY_EXPORTS=1"],
         render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_render_config(
-            rgbd=bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)), **_image_size(cfg, 40)),
+            rgbd=bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)), **_render_options(cfg, 40)),
     ),
     # GPU only: the gallery sim with uvs and textured materials (tests/test_render_textures.py);
     # same sources and flags, so it shares the gallery's simulator module
     "gallery_textured": SimDesc(
         name="gallery_textured",
         sources=[os.path.join(_ROOT, "gallery", "sim.cpp")],
-        num_exports=10,
+        num_exports=12,
         num_taskgraphs=1,
         inputs=[],
         outputs=[],
@@ -370,9 +378,10 @@ SIMS: Dict[str, SimDesc] = {
         pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
         oracle_extra=lambda cfg: [],
         defaults={"num_props": 100, "seed": 0, "resolution": 40, "rgbd": True, "bc7": False},
+        compile_flags=["-DGALLERY_ENTITY_EXPORTS=1"],
         render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_textured_render_config(
             rgbd=bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)),
-            bc7=bool(cfg.get("bc7", False)), **_image_size(cfg, 40)),
+            bc7=bool(cfg.get("bc7", False)), **_render_options(cfg, 40)),
     ),
     # GPU only: 145 bodies per world, past the per-world body cap (tests/test_cliffs.py)
     "balls_cliff": SimDesc(

@@ -26,6 +26,10 @@ void Sim::registerTypes(ECSRegistry &registry, const Config &)
     registry.exportColumn<Viewer, Rotation>((uint32_t)ExportID::ViewRot);
     registry.exportColumn<RaycastOutputArchetype, RGBOutputBuffer>((uint32_t)ExportID::RGB);
     registry.exportColumn<RaycastOutputArchetype, DepthOutputBuffer>((uint32_t)ExportID::Depth);
+#if defined(GALLERY_ENTITY_EXPORTS)
+    registry.exportColumn<Prop, Entity>((uint32_t)ExportID::PropEntity);
+    registry.exportColumn<RaycastOutputArchetype, SegmentationOutputBuffer>((uint32_t)ExportID::Segmentation);
+#endif
 }
 
 // props turn about z by a fixed small step (cos, sin of 0.02 rad as literals) and bob

@@ -26,10 +26,13 @@ using madrona::base::ObjectID;
 constexpr int32_t kNumViews = 2;
 constexpr int32_t kNumLights = 2;
 
+// PropEntity and Segmentation are exported when built with -DGALLERY_ENTITY_EXPORTS=1 (as the
+// fixtures are); without it the gallery exports the first ten slots only
 enum class ExportID : uint32_t {
     PropPos, PropRot, PropScale, PropObj, PropMat, PropColor,
     ViewPos, ViewRot,
     RGB, Depth,
+    PropEntity, Segmentation,
     NumExports,
 };
 

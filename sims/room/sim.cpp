@@ -69,6 +69,9 @@ void Sim::registerTypes(ECSRegistry &registry, const Config &)
         (uint32_t)ExportID::RenderDepth);
     registry.exportColumn<PhysicsEntity, Scale>((uint32_t)ExportID::BodyScale);
     registry.exportColumn<PhysicsEntity, ObjectID>((uint32_t)ExportID::BodyObject);
+    registry.exportColumn<Agent, Entity>((uint32_t)ExportID::AgentEntity);
+    registry.exportColumn<render::RaycastOutputArchetype, render::SegmentationOutputBuffer>(
+        (uint32_t)ExportID::RenderSegmentation);
 #endif
 }
 

@@ -61,6 +61,8 @@ enum class ExportID : uint32_t {
     RenderDepth,
     BodyScale,
     BodyObject,
+    AgentEntity,
+    RenderSegmentation,
 #endif
     NumExports,
 };
