@@ -89,8 +89,13 @@ typedef struct mb2_material_view {
  * [render_height][render_width] int32: the Entity id (without its generation) of
  * the renderable that the pixel's primary ray hits first, -1 where the ray hits
  * nothing, so -1 exactly where the depth is 0; 0 (zero-initialised) leaves it out.
- * mb2_executor_create returns NULL and mb2_last_error() says why when any of this
- * does not hold (segmentation is 0 or 1). */
+ * projection (not in the reference) is the camera model of every view: 0
+ * (zero-initialised) the pinhole; 1 a 360-degree equirectangular panorama, whose
+ * columns span azimuth -180..180 degrees (0 = the view's forward, columns turning
+ * toward +u as the pinhole's do) and whose rows span the vertical field of view
+ * evenly in elevation; depth is then the distance along the unit ray (a lidar's
+ * range).  mb2_executor_create returns NULL and mb2_last_error() says why when any
+ * of this does not hold (segmentation and projection are 0 or 1). */
 typedef struct mb2_render_config {
     uint32_t render_mode;          /* 0 RGBD, 1 Depth */
     mb2_mesh_bvh_view geo_bvh_data;
@@ -101,6 +106,7 @@ typedef struct mb2_render_config {
     uint32_t render_width;         /* columns per view, or 0 */
     uint32_t render_height;        /* rows per view, or 0 */
     uint32_t segmentation;         /* 1: per-pixel entity ids, 0: none */
+    uint32_t projection;           /* 0 pinhole, 1 panorama */
 } mb2_render_config;
 
 /* Triangle mesh -> BLAS.  Role of MeshBVHBuilder (src/common/mesh_bvh_builder.cpp,

@@ -361,10 +361,12 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
         return false;
     }
     if (rc) {
-        // the image size and the segmentation flag are checked before any CUDA call or allocation
-        uint32_t width, height, segmentation;
+        // the image size, the segmentation flag and the projection are checked before any CUDA
+        // call or allocation
+        uint32_t width, height, segmentation, projection;
         std::string err;
-        if (!renderImageSize(rc, &width, &height, &err) || !renderSegmentation(rc, &segmentation, &err)) {
+        if (!renderImageSize(rc, &width, &height, &err) || !renderSegmentation(rc, &segmentation, &err) ||
+            !renderProjection(rc, &projection, &err)) {
             setError(err);
             return false;
         }

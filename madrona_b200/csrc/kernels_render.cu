@@ -29,6 +29,7 @@
 // -> watertight ray / triangle test; materials (override colour / material
 // table, material textures sampled at the final hit's uv), lights with shadow
 // rays, RGBA8 + f32 depth (+ the hit entity's id when the config asks for segmentation).
+// Views are pinholes, or with projection = 1 360-degree equirectangular panoramas.
 //
 // Image formation follows the reference's CUDA ray tracer
 // (src/mw/device/bvh_raycast.cpp): ray generation :58-88, object-space ray and
@@ -1264,12 +1265,59 @@ __device__ __forceinline__ bool boxOutside(const float *lo, const float *hi, Vec
     return reach < 0.f;
 }
 
+// ---- panoramas (mb2_render_config::projection = 1) ---------------------------------------------
+// Pixel (px, py) of a W x H panorama looks at azimuth theta = s 2 pi ((px + 0.5) / W - 0.5) and
+// elevation phi = 2 phi_max ((py + 0.5) / H - 0.5), phi_max = atan(h) and s = sign(h), in the
+// view's (forward, u, vv) frame.  The flat path's culls are cone tests in place of the pinhole's
+// planes; their slacks absorb fp32 rounding (tests/test_raycast_panorama_model.py).
+constexpr float kPi = 3.14159265358979f;
+constexpr float kPanoBandSlack = 1e-5f;     // radians of elevation (view cull)
+constexpr float kPanoConeSlack = 1e-5f;     // of the cosine of the angle (tile cull)
+
+// The box (lo, hi relative to the view origin) as seen from the origin: the unit direction to
+// its centre and the half-angle beta of its bounding sphere (the sphere through its corners).
+// A sphere that holds the origin may be seen in any direction: beta = pi.
+struct PanoCone {
+    float dir[3];
+    float beta, sinb, cosb;
+};
+
+__device__ __forceinline__ PanoCone panoCone(const float *lo, const float *hi)
+{
+    const float bx = 0.5f * (lo[0] + hi[0]), by = 0.5f * (lo[1] + hi[1]), bz = 0.5f * (lo[2] + hi[2]);
+    const float hx = 0.5f * (hi[0] - lo[0]), hy = 0.5f * (hi[1] - lo[1]), hz = 0.5f * (hi[2] - lo[2]);
+    const float r = sqrtf(hx * hx + hy * hy + hz * hz);
+    const float d = sqrtf(bx * bx + by * by + bz * bz);
+    PanoCone c;
+    if (!(d > r)) {
+        c.dir[0] = 0.f; c.dir[1] = 0.f; c.dir[2] = 0.f;
+        c.beta = kPi; c.sinb = 0.f; c.cosb = -1.f;
+        return c;
+    }
+    const float inv = 1.f / d;
+    c.dir[0] = bx * inv; c.dir[1] = by * inv; c.dir[2] = bz * inv;
+    c.sinb = fminf(r * inv, 1.f);
+    c.cosb = sqrtf(fmaxf(1.f - c.sinb * c.sinb, 0.f));
+    c.beta = asinf(c.sinb);
+    return c;
+}
+
+// Does the cone lie wholly above or below the elevations |phi| <= band?  Elevation is the
+// angle from the vv = 0 plane, which moves by at most beta across the cone.
+__device__ __forceinline__ bool panoOutsideBand(const PanoCone &c, Vector3 vv, float band)
+{
+    if (c.beta >= kPi) return false;
+    const float e = asinf(fminf(fmaxf(c.dir[0] * vv.x + c.dir[1] * vv.y + c.dir[2] * vv.z, -1.f), 1.f));
+    return e - c.beta > band + kPanoBandSlack || e + c.beta < -band - kPanoBandSlack;
+}
+
 constexpr int kRaycastMinBlocks = 3;   // blocks per SM the ray caster is compiled for
 // FLAT: this launch traces the views of worlds with <= kFlatInstances instances, the other
 // instantiation the rest (a view belongs to exactly one of the two launches).
 // MATERIALS: the render config has a material table.  Without one no hit can name a texture,
-// so the texture code is left out and such scenes keep the code they had before textures
-template <bool FLAT, bool MATERIALS>
+// so the texture code is left out and such scenes keep the code they had before textures.
+// PANORAMA: the render config's projection is the 360-degree panorama (else the pinhole).
+template <bool FLAT, bool MATERIALS, bool PANORAMA>
 __global__ void __launch_bounds__(256, kRaycastMinBlocks)
 renderRaycastKernel(EngineState *Sp)
 {
@@ -1296,6 +1344,7 @@ renderRaycastKernel(EngineState *Sp)
     __shared__ FlatInstance s_list[kFlatInstances];      // sorted front to back
     __shared__ FlatInstance s_unsorted[kFlatInstances];
     __shared__ float s_key[kFlatInstances];
+    __shared__ PanoCone s_cone[PANORAMA ? kFlatInstances : 1];     // s_list's cones (panoramas)
 
     for (i32 v = blockIdx.y; v < num_views; v += gridDim.y) {
         const RenderView view = R.views[v];
@@ -1320,11 +1369,14 @@ renderRaycastKernel(EngineState *Sp)
         const Vector3 forward = look_at.normalize();
         const Vector3 u = rot.inv().rotateVec({ 1, 0, 0 });
         const Vector3 vv = cross(forward, u).normalize();
+        // panoramas: the rows span elevations -phi_max .. phi_max (signed like h)
+        const float phi_max = PANORAMA ? atanf(h) : 0.f;
 
         // ---- stage the world's instances, front to back, culled against the view frustum
         __syncthreads();        // the previous view's rays are done with the list
         if (flat) {
             const int i = (int)threadIdx.x;
+            PanoCone cone;
             if (i < num_instances) {
                 FlatInstance &fi = s_unsorted[i];
                 const RenderInstance &inst = instances[i];
@@ -1348,12 +1400,19 @@ renderRaycastKernel(EngineState *Sp)
                     const float gap = fmaxf(fmaxf(lo[a], -hi[a]), 0.f);    // distance to the box on this axis
                     dist2 += gap * gap;
                 }
-                // whole-view frustum: |a| <= h (W/H) c, |b| <= h c, c >= 0 in the (u, vv, forward) frame
-                const float pad_u = fabsf(h) * aspect * (1.f + 2.f / (float)W);
-                const float pad_v = fabsf(h) * (1.f + 2.f / (float)H);
-                const bool outside = boxOutside(lo, hi, forward) ||
-                    boxOutside(lo, hi, u + pad_u * forward) || boxOutside(lo, hi, pad_u * forward - u) ||
-                    boxOutside(lo, hi, vv + pad_v * forward) || boxOutside(lo, hi, pad_v * forward - vv);
+                bool outside;
+                if (PANORAMA) {
+                    // every azimuth is seen: only the elevation band can leave a box out
+                    cone = panoCone(lo, hi);
+                    outside = panoOutsideBand(cone, vv, fabsf(phi_max));
+                } else {
+                    // whole-view frustum: |a| <= h (W/H) c, |b| <= h c, c >= 0 in the (u, vv, forward) frame
+                    const float pad_u = fabsf(h) * aspect * (1.f + 2.f / (float)W);
+                    const float pad_v = fabsf(h) * (1.f + 2.f / (float)H);
+                    outside = boxOutside(lo, hi, forward) ||
+                        boxOutside(lo, hi, u + pad_u * forward) || boxOutside(lo, hi, pad_u * forward - u) ||
+                        boxOutside(lo, hi, vv + pad_v * forward) || boxOutside(lo, hi, pad_v * forward - vv);
+                }
                 fi.inView = outside ? 0 : 1;
                 s_key[i] = dist2;
             }
@@ -1369,6 +1428,7 @@ renderRaycastKernel(EngineState *Sp)
                 u32 *dst = (u32 *)&s_list[rank];
 #pragma unroll
                 for (int k = 0; k < (int)(sizeof(FlatInstance) / 4); k++) dst[k] = src[k];
+                if (PANORAMA) s_cone[rank] = cone;
             }
             __syncthreads();
         }
@@ -1391,7 +1451,37 @@ renderRaycastKernel(EngineState *Sp)
 
             // ---- instances that reach into this tile's sub-frustum (warp-uniform mask)
             unsigned long long tile_mask = 0;
-            if (flat) {
+            if (flat && PANORAMA) {
+                // the ray of the middle of the tile's pixel centres, c, and alpha: half the
+                // azimuth span plus half the elevation span of those centres, each a quarter
+                // pixel wider.  Every ray of the tile is within alpha of c (along the meridian,
+                // then along the parallel), so a box whose centre is farther than alpha + beta
+                // from c (beta: its cone's half-angle) is missed by all of them.
+                const u32 nx = min(tile_w, W - tx0), ny = min(tile_h, H - ty0);
+                const float s = h < 0.f ? -1.f : 1.f;
+                const float theta_c = s * (2.f * kPi) * (((float)tx0 + 0.5f * (float)nx) / (float)W - 0.5f);
+                const float phi_c = 2.f * phi_max * (((float)ty0 + 0.5f * (float)ny) / (float)H - 0.5f);
+                const float alpha = (0.5f * (float)(nx - 1) + 0.25f) * (2.f * kPi / (float)W) +
+                                    (0.5f * (float)(ny - 1) + 0.25f) * (2.f * fabsf(phi_max) / (float)H);
+                const float cp = cosf(phi_c);
+                const Vector3 c = cp * (cosf(theta_c) * forward + sinf(theta_c) * u) + sinf(phi_c) * vv;
+                const float cos_a = cosf(alpha), sin_a = sinf(alpha);
+#pragma unroll
+                for (int half = 0; half < kFlatInstances / 32; half++) {
+                    const int k = half * 32 + lane;
+                    bool keep = false;
+                    if (k < num_instances) {
+                        const FlatInstance &fi = s_list[k];
+                        const PanoCone &cn = s_cone[k];
+                        // angle(c, box) <= alpha + beta  <=>  cos(angle) >= cos(alpha + beta) below pi
+                        keep = fi.mesh >= 0 && fi.inView &&
+                            (alpha + cn.beta >= kPi ||
+                             c.x * cn.dir[0] + c.y * cn.dir[1] + c.z * cn.dir[2] >=
+                                 cos_a * cn.cosb - sin_a * cn.sinb - kPanoConeSlack);
+                    }
+                    tile_mask |= (unsigned long long)__ballot_sync(0xffffffffu, keep) << (32 * half);
+                }
+            } else if (flat) {
                 const float inv_w = 1.f / (float)W, inv_h = 1.f / (float)H;
                 // tile edges, a quarter pixel wider on each axis (the rays go through pixel centres)
                 const float a0 = ((float)tx0 * inv_w - 0.25f * inv_w - 0.5f) * viewport_w;
@@ -1416,13 +1506,25 @@ renderRaycastKernel(EngineState *Sp)
             }
             if (px >= W || py >= H) continue;
 
-            // ---- primary ray (bvh_raycast.cpp:58-88, with viewport_width = viewport_height * W / H)
-            const Vector3 horizontal = u * viewport_w;
-            const Vector3 vertical = vv * viewport;
-            const Vector3 lower_left = ray_start - horizontal / 2 - vertical / 2 + forward;
-            const float pu = ((float)px + 0.5f) / (float)W;
-            const float pv = ((float)py + 0.5f) / (float)H;
-            Vector3 ray_dir = lower_left + pu * horizontal + pv * vertical - ray_start;
+            Vector3 ray_dir;
+            if (PANORAMA) {
+                // ---- primary ray of a panorama: azimuth over the columns (0 = forward, the
+                // seam behind the camera), elevation over the rows; a mirrored view (h < 0)
+                // mirrors both, as the pinhole does
+                const float s = h < 0.f ? -1.f : 1.f;
+                const float theta = s * (2.f * kPi) * (((float)px + 0.5f) / (float)W - 0.5f);
+                const float phi = 2.f * phi_max * (((float)py + 0.5f) / (float)H - 0.5f);
+                const float cp = cosf(phi);
+                ray_dir = cp * (cosf(theta) * forward + sinf(theta) * u) + sinf(phi) * vv;
+            } else {
+                // ---- primary ray (bvh_raycast.cpp:58-88, with viewport_width = viewport_height * W / H)
+                const Vector3 horizontal = u * viewport_w;
+                const Vector3 vertical = vv * viewport;
+                const Vector3 lower_left = ray_start - horizontal / 2 - vertical / 2 + forward;
+                const float pu = ((float)px + 0.5f) / (float)W;
+                const float pv = ((float)py + 0.5f) / (float)H;
+                ray_dir = lower_left + pu * horizontal + pv * vertical - ray_start;
+            }
             ray_dir = ray_dir.normalize();
 
             const RayHit first = flat
@@ -1593,10 +1695,22 @@ bool renderSegmentation(const mb2_render_config *rc, u32 *on, std::string *err)
     return true;
 }
 
+// The camera model of a render config (0 pinhole, 1 panorama; else invalid).
+bool renderProjection(const mb2_render_config *rc, u32 *projection, std::string *err)
+{
+    if (rc->projection > 1) {
+        *err = "projection = " + std::to_string(rc->projection) + " is not 0 (pinhole) or 1 (panorama)";
+        return false;
+    }
+    *projection = rc->projection;
+    return true;
+}
+
 bool renderHostCreate(Executor *ex, const mb2_render_config *rc, std::string *err)
 {
-    u32 width = 0, height = 0, segmentation = 0;
-    if (rc && (!renderImageSize(rc, &width, &height, err) || !renderSegmentation(rc, &segmentation, err))) return false;
+    u32 width = 0, height = 0, segmentation = 0, projection = 0;
+    if (rc && (!renderImageSize(rc, &width, &height, err) || !renderSegmentation(rc, &segmentation, err) ||
+               !renderProjection(rc, &projection, err))) return false;
     RenderHost *rh = new RenderHost();
     ex->render = rh;
     memset(&rh->hRender, 0, sizeof(RenderState));
@@ -1617,6 +1731,7 @@ bool renderHostCreate(Executor *ex, const mb2_render_config *rc, std::string *er
         R.height = height;
         R.rgbd = rc->render_mode == 0 ? 1u : 0u;
         R.segmentation = segmentation;
+        R.projection = projection;
         R.nearPlane = rc->near_plane;
         R.farPlane = rc->far_plane;
         // device pointers, adopted as they are (the reference frees them in its
@@ -1877,12 +1992,20 @@ LaunchGraph *physicsBuildRenderGraph(Executor *ex, std::string *err)
     // the live view count: one block per capacity row cost 76 us of empty-block scheduling at
     // 1024 worlds); 8 rounds of resident blocks keep the tail short
     const unsigned view_blocks = (unsigned)std::max(1, std::min(R.maxViews, ex->numSMs * kRaycastMinBlocks * 8));
-    if (R.materials) {
-        renderRaycastKernel<true, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
-        renderRaycastKernel<false, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+    if (R.projection == 1) {
+        if (R.materials) {
+            renderRaycastKernel<true, true, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+            renderRaycastKernel<false, true, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+        } else {
+            renderRaycastKernel<true, false, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+            renderRaycastKernel<false, false, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+        }
+    } else if (R.materials) {
+        renderRaycastKernel<true, true, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+        renderRaycastKernel<false, true, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
     } else {
-        renderRaycastKernel<true, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
-        renderRaycastKernel<false, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+        renderRaycastKernel<true, false, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+        renderRaycastKernel<false, false, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
     }
     launchStatusCopy(ex, ex->stream);
     cudaError_t e = cudaStreamEndCapture(ex->stream, &g->graph);

@@ -23,6 +23,8 @@ LaunchGraph *physicsBuildRenderGraph(Executor *ex, std::string *err);
 bool renderImageSize(const mb2_render_config *rc, uint32_t *width, uint32_t *height, std::string *err);
 // whether a render config asks for the segmentation output, or false and why it is invalid
 bool renderSegmentation(const mb2_render_config *rc, uint32_t *on, std::string *err);
+// the camera model of a render config (0 pinhole, 1 panorama), or false and why it is invalid
+bool renderProjection(const mb2_render_config *rc, uint32_t *projection, std::string *err);
 bool renderHostCreate(Executor *ex, const mb2_render_config *rc, std::string *err);
 bool renderHostAfterRegistry(Executor *ex, std::string *err);
 void renderHostDestroy(Executor *ex);

@@ -87,6 +87,7 @@ struct RenderState {
     const RenderMaterial *materials;   // device, == materialData.materials (may be null)
     u32 debugHits;                  // MADRONA_B200_RENDER_DEBUG: keep (instance, triangle) per pixel
     u32 segmentation;               // 1: each view also gets an i32 entity id per pixel
+    u32 projection;                 // 0: pinhole, 1: 360-degree equirectangular panorama
 
     // ---- written by the device-side RenderingSystem::registerTypes
     u32 registered;

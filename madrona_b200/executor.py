@@ -117,7 +117,7 @@ class _MaterialViewC(ctypes.Structure):      # == render::MaterialData
     ]
 
 
-class _RenderConfigC(ctypes.Structure):      # == madrona::CudaBatchRenderConfig + image size + outputs
+class _RenderConfigC(ctypes.Structure):      # == madrona::CudaBatchRenderConfig + image size + outputs + projection
     _fields_ = [
         ("render_mode", ctypes.c_uint32),
         ("geo_bvh_data", _MeshBVHViewC),
@@ -130,6 +130,8 @@ class _RenderConfigC(ctypes.Structure):      # == madrona::CudaBatchRenderConfig
         ("render_height", ctypes.c_uint32),
         # 1: per view one more output, int32 [height][width]: the hit entity's id, -1 on a miss
         ("segmentation", ctypes.c_uint32),
+        # camera model of every view: 0 pinhole, 1 360-degree equirectangular panorama
+        ("projection", ctypes.c_uint32),
     ]
 
 

@@ -160,6 +160,16 @@ struct RenderOutputs {
     bool segmentation;
 };
 
+// The camera model of every view, for the MWCudaExecutor constructor overload that takes one.
+// Pinhole: the reference's camera.  Panorama: each view's image covers 360 degrees of azimuth
+// across its columns (the middle looks along the view's forward, the seam is behind it) and
+// the vertical field of view across its rows, evenly spaced in elevation; the depth output is
+// the distance along the unit ray, a lidar's range.
+enum class RenderProjection : uint32_t {
+    Pinhole = 0,
+    Panorama = 1,
+};
+
 // A device-memory snapshot of an executor's simulation state (include/madrona_b200.h),
 // made by MWCudaExecutor::snapshot().  save() / restore() are one kernel launch each on
 // `strm` (by default the executor's stream) and never synchronize the host; stepping after
@@ -248,7 +258,7 @@ public:
                        Optional<CudaBatchRenderConfig>::none())
     {
         create(state_cfg, compile_cfg, cu_ctx, render_cfg, ::madrona_b200::RenderImageSize { 0, 0 },
-               ::madrona_b200::RenderOutputs { false });
+               ::madrona_b200::RenderOutputs { false }, ::madrona_b200::RenderProjection::Pinhole);
     }
 
     // Not in the reference: the batch renderer's images are image_size.width columns by
@@ -257,7 +267,8 @@ public:
                    CUcontext cu_ctx, const Optional<CudaBatchRenderConfig> &render_cfg,
                    const ::madrona_b200::RenderImageSize &image_size)
     {
-        create(state_cfg, compile_cfg, cu_ctx, render_cfg, image_size, ::madrona_b200::RenderOutputs { false });
+        create(state_cfg, compile_cfg, cu_ctx, render_cfg, image_size, ::madrona_b200::RenderOutputs { false },
+               ::madrona_b200::RenderProjection::Pinhole);
     }
 
     // Not in the reference: the image size as above (RenderImageSize { 0, 0 }: the
@@ -267,7 +278,19 @@ public:
                    const ::madrona_b200::RenderImageSize &image_size,
                    const ::madrona_b200::RenderOutputs &outputs)
     {
-        create(state_cfg, compile_cfg, cu_ctx, render_cfg, image_size, outputs);
+        create(state_cfg, compile_cfg, cu_ctx, render_cfg, image_size, outputs,
+               ::madrona_b200::RenderProjection::Pinhole);
+    }
+
+    // Not in the reference: the image size and outputs as above, and the camera model of
+    // every view (RenderProjection::Panorama: 360-degree equirectangular views).
+    MWCudaExecutor(const StateConfig &state_cfg, const CompileConfig &compile_cfg,
+                   CUcontext cu_ctx, const Optional<CudaBatchRenderConfig> &render_cfg,
+                   const ::madrona_b200::RenderImageSize &image_size,
+                   const ::madrona_b200::RenderOutputs &outputs,
+                   ::madrona_b200::RenderProjection projection)
+    {
+        create(state_cfg, compile_cfg, cu_ctx, render_cfg, image_size, outputs, projection);
     }
 
     MWCudaExecutor(MWCudaExecutor &&o) : h_(o.h_) { o.h_ = nullptr; }
@@ -340,7 +363,8 @@ private:
     void create(const StateConfig &state_cfg, const CompileConfig &compile_cfg, CUcontext cu_ctx,
                 const Optional<CudaBatchRenderConfig> &render_cfg,
                 const ::madrona_b200::RenderImageSize &image_size,
-                const ::madrona_b200::RenderOutputs &outputs)
+                const ::madrona_b200::RenderOutputs &outputs,
+                ::madrona_b200::RenderProjection projection)
     {
         mb2_state_config sc {
             state_cfg.worldInitPtr, state_cfg.numWorldInitBytes,
@@ -368,6 +392,7 @@ private:
             rc.render_width = image_size.width;
             rc.render_height = image_size.height;
             rc.segmentation = outputs.segmentation ? 1u : 0u;
+            rc.projection = (uint32_t)projection;
         }
         int gpu_id = mb2_device_of_context((void *)cu_ctx);
         h_ = mb2_executor_create(&sc, &cc, gpu_id, render_cfg.has_value() ? &rc : nullptr);

@@ -146,9 +146,11 @@ def _image_size(cfg, default_res):
 
 
 def _render_options(cfg, default_res):
-    """Keyword arguments for the render_assets builders: the image size, and `segmentation`
-    (per-pixel hit entity ids, off unless the fixture config sets it)."""
-    return dict(_image_size(cfg, default_res), segmentation=bool(cfg.get("segmentation", False)))
+    """Keyword arguments for the render_assets builders: the image size, `segmentation`
+    (per-pixel hit entity ids) and `panorama` (360-degree equirectangular views instead of
+    pinholes), both off unless the fixture config sets them."""
+    return dict(_image_size(cfg, default_res), segmentation=bool(cfg.get("segmentation", False)),
+                panorama=bool(cfg.get("panorama", False)))
 
 
 def _room_render_cfg(cfg):
