@@ -10,11 +10,13 @@
 #include "../../include/madrona_b200.h"
 #include "engine.hpp"
 #include "physics_host.hpp"
+#include "physics_state.h"
 
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <algorithm>
+#include <variant>
 #include <cxxabi.h>
 
 namespace mb2 {
@@ -101,11 +103,88 @@ static bool launch1(Executor *ex, cudaKernel_t k, unsigned grid, unsigned block)
     return true;
 }
 
-static uint64_t envU64(const char *name, uint64_t dflt)
+// ---- environment knobs ------------------------------------------------------
+
+// Unset means the default.  A set value must be valid, so that a typo fails executor creation
+// instead of running with a misread capacity: a boolean is exactly 0 or 1, an integer decimal
+// digits within its range, a path any non-empty string.
+bool parseKnobs(uint32_t num_worlds, Knobs *k, std::string *err)
 {
-    const char *v = getenv(name);
-    if (!v || !*v) return dflt;
-    return strtoull(v, nullptr, 10);
+    constexpr uint64_t kI32Max = INT32_MAX, kU64Max = UINT64_MAX;
+    struct Row {
+        const char *name;
+        std::variant<bool *, uint64_t *, std::string *> out;   // the kind: boolean, integer, path
+        std::string dflt;
+        uint64_t lo = 0, hi = 0;   // integers: the accepted range
+        const char *counts = "";   // integers: what the number counts, for the error message
+    };
+    const Row rows[] = {
+        { "MADRONA_B200_ROWS_PER_WORLD", &k->rowsPerWorld, "128", 1, kI32Max,
+          "initial rows per world of a dynamic table" },
+        { "MADRONA_B200_TABLE_GROWTH", &k->tableGrowth, "1" },
+        { "MADRONA_B200_TMP_BYTES", &k->tmpBytes, std::to_string(256ull << 20), 1, kU64Max,
+          "bytes of the tmp arena" },
+        { "MADRONA_B200_PERSIST_BYTES", &k->persistBytes,
+          std::to_string((64ull << 20) + (uint64_t)num_worlds * (24ull << 10)), 1, kU64Max,
+          "bytes of the persistent arena" },
+        { "MADRONA_B200_GRAPH_BRANCHES", &k->graphBranches, "1" },
+        { "MADRONA_B200_MAX_CANDIDATES_PER_WORLD", &k->maxCandidatesPerWorld, "256", 1, kI32Max,
+          "candidate pairs per world" },
+        { "MADRONA_B200_MAX_CONTACTS_PER_WORLD", &k->maxContactsPerWorld, "128", 1, kI32Max,
+          "contacts per world" },
+        { "MADRONA_B200_MAX_HULL_SIZE", &k->maxHullSize, std::to_string(kMinHullSizeCap),
+          kMinHullSizeCap, kMaxHullSizeCap, "vertices and faces per convex hull" },
+        { "MADRONA_B200_MAX_BODIES_PER_WORLD", &k->maxWorldBodies, std::to_string(kMinWorldBodiesCap),
+          kMinWorldBodiesCap, kMaxWorldBodiesCap, "rigid bodies per world" },
+        { "MADRONA_B200_RENDER_DEBUG", &k->renderDebug, "0" },
+        { "MADRONA_B200_FAST_MATH", &k->fastMath, "0" },
+        { "MADRONA_B200_NO_KERNEL_CACHE", &k->noKernelCache, "0" },
+        { "MADRONA_B200_KERNEL_CACHE_DIR", &k->kernelCacheDir, moduleDir() + "/_jit_cache" },
+    };
+    for (const Row &r : rows) {
+        const char *env = getenv(r.name);
+        const std::string v = env ? env : r.dflt;
+        const std::string got = ", got \"" + v + "\"";
+        if (bool *const *flag = std::get_if<bool *>(&r.out)) {
+            if (v != "0" && v != "1") {
+                *err = std::string(r.name) + " must be 0 or 1" + got;
+                return false;
+            }
+            **flag = v == "1";
+        } else if (uint64_t *const *num = std::get_if<uint64_t *>(&r.out)) {
+            uint64_t n = 0;
+            bool ok = !v.empty();
+            for (char c : v) {
+                const uint64_t d = (uint64_t)(c - '0');
+                if (c < '0' || c > '9' || n > (kU64Max - d) / 10) {   // not a digit, or overflow
+                    ok = false;
+                    break;
+                }
+                n = n * 10 + d;
+            }
+            if (!ok || n < r.lo || n > r.hi) {
+                *err = std::string(r.name) + " must be a number from " + std::to_string(r.lo) + " to " +
+                       std::to_string(r.hi) + " (" + r.counts + ")" + got;
+                return false;
+            }
+            **num = n;
+        } else {
+            if (v.empty()) {
+                *err = std::string(r.name) + " must be a non-empty path" + got;
+                return false;
+            }
+            *std::get<std::string *>(r.out) = v;
+        }
+    }
+    return true;
+}
+
+static bool jitCompileConfig(const mb2_compile_config *cc, const Knobs &k, JitModule *m, std::string *err)
+{
+    std::vector<std::string> sources, flags;
+    for (uint32_t i = 0; i < cc->num_user_sources; i++) sources.push_back(cc->user_sources[i]);
+    for (uint32_t i = 0; i < cc->num_user_compile_flags; i++) flags.push_back(cc->user_compile_flags[i]);
+    return jitCompile(sources, flags, (int)cc->opt_mode, k.fastMath, !k.noKernelCache, k.kernelCacheDir, m, err);
 }
 
 // ---- table allocation after registerTypes ---------------------------------
@@ -130,8 +209,8 @@ static bool allocateTables(Executor *ex)
         else {
             // wide rows (the ray caster's per-view image buffers) start with fewer rows per
             // world so the initial mapping fits an 80 GB card; growable tables double from there
-            uint64_t per_world = ex->rowsPerWorldHint;
-            if (ex->tableGrowth) {
+            uint64_t per_world = ex->knobs.rowsPerWorld;
+            if (ex->knobs.tableGrowth) {
                 uint64_t row_bytes = 0;
                 for (uint32_t c = 0; c < info.numUserComponents; c++) {
                     if (info.componentIDs[c] < S.numComponents) row_bytes += S.components[info.componentIDs[c]].numBytes;
@@ -154,7 +233,7 @@ static bool allocateTables(Executor *ex)
 
         // dynamic archetypes live in growable address ranges (up to 64x the initial
         // capacity, the row index stays a positive int32); fixed ones are W x max rows for good
-        const bool growable = ex->tableGrowth && !info.isSingleton && info.maxPerWorld == 0;
+        const bool growable = ex->knobs.tableGrowth && !info.isSingleton && info.maxPerWorld == 0;
         const uint64_t reserve_rows = std::min<uint64_t>(cap * 64, 0x7fffff00ull);
         if (growable) ex->columnRanges[a].resize(t.numColumns);
         ex->maxRows[a] = growable ? (int64_t)reserve_rows : (int64_t)cap;
@@ -216,7 +295,7 @@ static bool allocateTables(Executor *ex)
     S.initExpandBlocks = (int32_t)init_blocks;
     S.numEntitySlots = (int32_t)(init_blocks * kIDsPerCache);
     S.freeHead = ((u64)0 << 32) | (u32)kIDSentinel;
-    if (ex->tableGrowth) {
+    if (ex->knobs.tableGrowth) {
         std::string verr;
         if (!vmReserve(ex->gpu, &ex->entityRange, sizeof(EntitySlot) * 0x7fffff00ull, sizeof(EntitySlot) * ent_cap,
                        &verr)) {
@@ -229,8 +308,8 @@ static bool allocateTables(Executor *ex)
     }
     if (!devAlloc(ex, (void **)&S.idCaches, sizeof(IDCache) * W)) return false;
 
-    S.tmpCapacity = envU64("MADRONA_B200_TMP_BYTES", 256ull << 20);
-    S.persistCapacity = envU64("MADRONA_B200_PERSIST_BYTES", (64ull << 20) + (uint64_t)W * (24ull << 10));
+    S.tmpCapacity = ex->knobs.tmpBytes;
+    S.persistCapacity = ex->knobs.persistBytes;
     if (!devAlloc(ex, (void **)&S.tmpArena, S.tmpCapacity, false)) return false;
     if (!devAlloc(ex, (void **)&S.persistArena, S.persistCapacity)) return false;
     S.tmpOffset = 0;
@@ -284,7 +363,7 @@ bool growTable(Executor *ex, uint32_t a, int64_t new_cap, std::string *err)
 // without overflowing -- the worst case of a full reset before compaction).
 static bool growTablesFromStatus(Executor *ex)
 {
-    if (!ex->tableGrowth) return true;
+    if (!ex->knobs.tableGrowth) return true;
     EngineState &S = *ex->hState;
     for (uint32_t a = 0; a < S.numArchetypes && a < (uint32_t)kMaxArchetypes; a++) {
         if (ex->columnRanges[a].empty()) continue;
@@ -360,26 +439,11 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
         setError("too many exported buffers");
         return false;
     }
-    if (rc) {
-        // the image size, the segmentation flag and the projection are checked before any CUDA
-        // call or allocation
-        uint32_t width, height, segmentation, projection;
-        std::string err;
-        if (!renderImageSize(rc, &width, &height, &err) || !renderSegmentation(rc, &segmentation, &err) ||
-            !renderProjection(rc, &projection, &err)) {
-            setError(err);
-            return false;
-        }
-    }
-
-    {
-        // so are the hull-size and world-size knobs of the physics
-        int max_hull_size, max_world_bodies;
-        std::string err;
-        if (!physicsMaxHullSize(&max_hull_size, &err) || !physicsMaxWorldBodies(&max_world_bodies, &err)) {
-            setError(err);
-            return false;
-        }
+    // the knobs and the render config are checked before any CUDA call or allocation
+    std::string err;
+    if (!parseKnobs(sc->num_worlds, &ex->knobs, &err) || !renderParseConfig(rc, &ex->renderSettings, &err)) {
+        setError(err);
+        return false;
     }
 
     MB2_CUDA(cudaSetDevice(ex->gpu));
@@ -396,15 +460,9 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
     // cudaStreamCreate): work the caller queued on the legacy default stream --
     // torch's `actions.copy_(...)` -- is ordered before the step graph
     MB2_CUDA(cudaStreamCreate(&ex->stream));
-    ex->rowsPerWorldHint = envU64("MADRONA_B200_ROWS_PER_WORLD", 128);
-    ex->tableGrowth = envU64("MADRONA_B200_TABLE_GROWTH", 1) != 0;
 
     // ---- JIT the simulator
-    std::vector<std::string> sources, flags;
-    for (uint32_t i = 0; i < cc->num_user_sources; i++) sources.push_back(cc->user_sources[i]);
-    for (uint32_t i = 0; i < cc->num_user_compile_flags; i++) flags.push_back(cc->user_compile_flags[i]);
-    std::string err;
-    if (!jitCompile(sources, flags, (int)cc->opt_mode, &ex->jit, &err)) {
+    if (!jitCompileConfig(cc, ex->knobs, &ex->jit, &err)) {
         setError(err);
         return false;
     }
@@ -486,7 +544,7 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
         setError(err);
         return false;
     }
-    if (!physicsHostAfterRegistry(ex, rc, &err) || !renderHostAfterRegistry(ex, &err)) {
+    if (!physicsHostAfterRegistry(ex, &err) || !renderHostAfterRegistry(ex, &err)) {
         setError(err);
         return false;
     }
@@ -504,7 +562,7 @@ static bool createExecutor(Executor *ex, const mb2_state_config *sc,
         uint32_t st[2] = { 0, 0 };
         MB2_CUDA(cudaMemcpy(st, &ex->dState->errorFlags, sizeof(st), cudaMemcpyDeviceToHost));
         const bool table_overflow = (st[0] & ~(uint32_t)ErrEntityOverflow) == (uint32_t)ErrTableOverflow;
-        if (table_overflow && ex->tableGrowth && attempt < 12 &&
+        if (table_overflow && ex->knobs.tableGrowth && attempt < 12 &&
                 st[1] < S.numArchetypes && !ex->columnRanges[st[1]].empty()) {
             std::string gerr;
             if (!growTable(ex, st[1], (int64_t)S.tables[st[1]].capacity * 2, &gerr)) {
@@ -792,7 +850,7 @@ static LaunchGraph *buildGraph(Executor *ex, const uint32_t *ids, uint32_t n, co
             units.push_back(std::move(u));
         }
     }
-    const bool branches = envU64("MADRONA_B200_GRAPH_BRANCHES", 1) != 0;
+    const bool branches = ex->knobs.graphBranches;
 
     cudaError_t e = cudaStreamBeginCapture(ex->stream, cudaStreamCaptureModeThreadLocal);
     if (e != cudaSuccess) {
@@ -1218,7 +1276,7 @@ int mb2_run_async(mb2_executor *exec, mb2_launch_graph *graph, void *cuda_stream
         return 1;
     }
     // an idle executor can act on the status its last graph published (table growth)
-    if ((cudaStream_t)cuda_stream != ex->stream && ex->tableGrowth &&
+    if ((cudaStream_t)cuda_stream != ex->stream && ex->knobs.tableGrowth &&
             cudaStreamQuery((cudaStream_t)cuda_stream) == cudaSuccess && cudaStreamQuery(ex->stream) == cudaSuccess) {
         if (ex->hStatus[0] == 0 && !growTablesFromStatus(ex)) return 1;
     }
@@ -1361,12 +1419,10 @@ void mb2_snapshot_destroy(mb2_snapshot *snap) { snapshotDestroy((Snapshot *)snap
 int mb2_jit_precompile(const mb2_compile_config *cc)
 {
     g_last_error.clear();
-    std::vector<std::string> sources, flags;
-    for (uint32_t i = 0; i < cc->num_user_sources; i++) sources.push_back(cc->user_sources[i]);
-    for (uint32_t i = 0; i < cc->num_user_compile_flags; i++) flags.push_back(cc->user_compile_flags[i]);
+    Knobs knobs;
     JitModule m;
     std::string err;
-    if (!jitCompile(sources, flags, (int)cc->opt_mode, &m, &err)) {
+    if (!parseKnobs(0, &knobs, &err) || !jitCompileConfig(cc, knobs, &m, &err)) {
         setError(err);
         return 1;
     }

@@ -16,6 +16,33 @@ struct SortScratch;   // kernels_sort.cu
 struct PhysicsHost;   // kernels_physics.cu
 struct RenderHost;    // kernels_render.cu
 
+// The MADRONA_B200_* environment variables that configure an executor, as parseKnobs read them
+struct Knobs {
+    uint64_t rowsPerWorld;             // ROWS_PER_WORLD: initial rows per world of a dynamic table
+    uint64_t tmpBytes, persistBytes;   // TMP_BYTES, PERSIST_BYTES: the two arenas
+    uint64_t maxCandidatesPerWorld;    // MAX_CANDIDATES_PER_WORLD
+    uint64_t maxContactsPerWorld;      // MAX_CONTACTS_PER_WORLD
+    uint64_t maxHullSize;              // MAX_HULL_SIZE
+    uint64_t maxWorldBodies;           // MAX_BODIES_PER_WORLD
+    bool tableGrowth;                  // TABLE_GROWTH
+    bool graphBranches;                // GRAPH_BRANCHES
+    bool fastMath;                     // FAST_MATH
+    bool noKernelCache;                // NO_KERNEL_CACHE
+    bool renderDebug;                  // RENDER_DEBUG
+    std::string kernelCacheDir;        // KERNEL_CACHE_DIR
+};
+
+// Reads every knob from the environment (num_worlds sizes the persistent arena's default).
+// False, and in *err the knob, what it accepts and what it got, on the first malformed value.
+bool parseKnobs(uint32_t num_worlds, Knobs *k, std::string *err);
+
+// What an executor's render config asks of the ray caster (all 0 without one)
+struct RenderSettings {
+    uint32_t width = 0, height = 0;
+    uint32_t segmentation = 0;   // 1: the per-pixel entity id output
+    uint32_t projection = 0;     // 0 pinhole, 1 panorama
+};
+
 struct Executor {
     int gpu = 0;
     int numSMs = 132;
@@ -41,12 +68,12 @@ struct Executor {
     PhysicsHost *physics = nullptr;
     RenderHost *render = nullptr;
 
-    uint64_t rowsPerWorldHint = 64;
+    Knobs knobs;                     // read and checked before any CUDA call
+    RenderSettings renderSettings;   // likewise, from the render config
 
     // ---- growable storage (vm_alloc.hpp): dynamic archetypes' columns and their sort
     // twins, the sort's key / index / look-back scratch and the entity store keep their
-    // base address and get more physical memory between steps
-    bool tableGrowth = true;                                   // MADRONA_B200_TABLE_GROWTH
+    // base address and get more physical memory between steps (unless knobs.tableGrowth is off)
     std::vector<VMRange> columnRanges[kMaxArchetypes];         // [archetype][column]; empty: fixed table
     std::vector<VMRange> twinRanges[kMaxArchetypes];
     int64_t maxRows[kMaxArchetypes] = {};                      // most rows a table can grow to

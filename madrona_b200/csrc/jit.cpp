@@ -188,15 +188,10 @@ static bool pairKernels(JitModule *m, const std::vector<std::string> &kerns,
 
 // ---- compile ---------------------------------------------------------------
 
-static std::string cacheDir()
-{
-    if (const char *env = getenv("MADRONA_B200_KERNEL_CACHE_DIR")) return env;
-    return moduleDir() + "/_jit_cache";
-}
-
 bool jitCompile(const std::vector<std::string> &sources,
                 const std::vector<std::string> &user_flags,
-                int opt_mode, JitModule *out, std::string *err)
+                int opt_mode, bool fast_math, bool use_cache, const std::string &cache_dir,
+                JitModule *out, std::string *err)
 {
     const std::string mod = moduleDir();
     const std::string dev_inc = mod + "/device";
@@ -205,8 +200,6 @@ bool jitCompile(const std::vector<std::string> &sources,
     std::string cuda_inc = "/usr/local/cuda/include";
     if (const char *env = getenv("CUDA_HOME")) cuda_inc = std::string(env) + "/include";
 
-    bool fast_math = false;
-    if (const char *env = getenv("MADRONA_B200_FAST_MATH")) fast_math = env[0] == '1';
     if (const char *env = getenv("MADRONA_MWGPU_FORCE_DEBUG")) {
         if (env[0] == '1') opt_mode = 2;
     }
@@ -280,12 +273,8 @@ bool jitCompile(const std::vector<std::string> &sources,
 
     char hex[32];
     snprintf(hex, sizeof(hex), "%016llx", (unsigned long long)h);
-    const std::string cache_dir = cacheDir();
     const std::string cache_path = cache_dir + "/" + hex + ".cubin";
     out->cachePath = cache_path;
-
-    bool use_cache = true;
-    if (const char *env = getenv("MADRONA_B200_NO_KERNEL_CACHE")) use_cache = env[0] != '1';
 
     std::string cached;
     if (use_cache && readFile(cache_path, &cached) && !cached.empty()) {

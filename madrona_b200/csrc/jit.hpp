@@ -18,8 +18,10 @@ struct JitModule {
 
 std::string moduleDir();
 
+// fast_math: FMA contraction on; use_cache: look the cubin up in and store it to cache_dir
 bool jitCompile(const std::vector<std::string> &sources,
                 const std::vector<std::string> &user_flags,
-                int opt_mode, JitModule *out, std::string *err);
+                int opt_mode, bool fast_math, bool use_cache, const std::string &cache_dir,
+                JitModule *out, std::string *err);
 
 }

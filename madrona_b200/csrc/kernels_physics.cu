@@ -3028,50 +3028,12 @@ bool physicsHostCreate(Executor *ex, std::string *err)
     return true;
 }
 
-static uint64_t envU64p(const char *name, uint64_t dflt)
-{
-    const char *v = getenv(name);
-    return (v && *v) ? strtoull(v, nullptr, 10) : dflt;
-}
-
-bool physicsMaxHullSize(int *size, std::string *err)
-{
-    *size = kMinHullSizeCap;
-    const char *v = getenv("MADRONA_B200_MAX_HULL_SIZE");
-    if (!v || !*v) return true;
-    char *end = nullptr;
-    const long n = strtol(v, &end, 10);
-    if (*end != '\0' || n < kMinHullSizeCap || n > kMaxHullSizeCap) {
-        *err = "MADRONA_B200_MAX_HULL_SIZE must be a number from " + std::to_string(kMinHullSizeCap) + " to " +
-               std::to_string(kMaxHullSizeCap) + " (vertices and faces per convex hull), got \"" + v + "\"";
-        return false;
-    }
-    *size = (int)n;
-    return true;
-}
-
-bool physicsMaxWorldBodies(int *bodies, std::string *err)
-{
-    *bodies = kMinWorldBodiesCap;
-    const char *v = getenv("MADRONA_B200_MAX_BODIES_PER_WORLD");
-    if (!v) return true;
-    char *end = nullptr;
-    const long n = strtol(v, &end, 10);
-    if (!*v || *end != '\0' || n < kMinWorldBodiesCap || n > kMaxWorldBodiesCap) {
-        *err = "MADRONA_B200_MAX_BODIES_PER_WORLD must be a number from " + std::to_string(kMinWorldBodiesCap) +
-               " to " + std::to_string(kMaxWorldBodiesCap) + " (rigid bodies per world), got \"" + v + "\"";
-        return false;
-    }
-    *bodies = (int)n;
-    return true;
-}
-
 static size_t largeStageBytes(int max_hull_size)
 {
     return (size_t)kLargeWarps * max_hull_size * kLargeStageBytesPerEntry;
 }
 
-bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::string *err)
+bool physicsHostAfterRegistry(Executor *ex, std::string *err)
 {
     PhysicsHost *ph = ex->physics;
     EngineState &S = *ex->hState;
@@ -3106,8 +3068,8 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::stri
     }
     P.jointCol = S.columnLookup[P.jointArchetype][P.cidJointConstraint];
 
-    P.maxCandidatesPerWorld = (i32)envU64p("MADRONA_B200_MAX_CANDIDATES_PER_WORLD", 256);
-    P.maxContactsPerWorld = (i32)envU64p("MADRONA_B200_MAX_CONTACTS_PER_WORLD", 128);
+    P.maxCandidatesPerWorld = (i32)ex->knobs.maxCandidatesPerWorld;
+    P.maxContactsPerWorld = (i32)ex->knobs.maxContactsPerWorld;
     const size_t W = S.numWorlds;
     auto alloc = [&](void **p, size_t bytes) {
         if (cudaMalloc(p, bytes) != cudaSuccess) return false;
@@ -3136,8 +3098,7 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::stri
         return false;
     }
     // hulls past the staging caps: the third work list and its kernel's shared memory
-    int max_hull_size = kMinHullSizeCap;
-    if (!physicsMaxHullSize(&max_hull_size, err)) return false;
+    const int max_hull_size = (int)ex->knobs.maxHullSize;
     P.maxHullSize = max_hull_size;
     if (max_hull_size > kMinHullSizeCap) {
         if (!alloc_list(P.largePairs, 2) ||
@@ -3154,8 +3115,7 @@ bool physicsHostAfterRegistry(Executor *ex, const mb2_render_config *, std::stri
     }
     // worlds past 128 bodies: their work list and the global contact level table (4 bytes per
     // world and body slot)
-    int max_world_bodies = kMinWorldBodiesCap;
-    if (!physicsMaxWorldBodies(&max_world_bodies, err)) return false;
+    const int max_world_bodies = (int)ex->knobs.maxWorldBodies;
     P.maxWorldBodies = max_world_bodies;
     if (max_world_bodies > kMinWorldBodiesCap) {
         P.largeWorlds.counters = pair_counters + 3;

@@ -1660,10 +1660,12 @@ static std::vector<LightCarrierArchetype> &lightCarriers(Executor *ex)
     return all.back().second;
 }
 
-// The image size a render config asks for: render_width x render_height when both are set,
-// else the render_resolution square.
-bool renderImageSize(const mb2_render_config *rc, u32 *width, u32 *height, std::string *err)
+// The image is render_width x render_height when both are set, else the render_resolution
+// square; segmentation and projection are 0 or 1.
+bool renderParseConfig(const mb2_render_config *rc, RenderSettings *out, std::string *err)
 {
+    *out = RenderSettings();
+    if (!rc) return true;
     const u32 res = rc->render_resolution, w = rc->render_width, h = rc->render_height;
     if ((w == 0) != (h == 0)) {
         *err = "render_width and render_height must be set together (both 0: a render_resolution square)";
@@ -1674,43 +1676,28 @@ bool renderImageSize(const mb2_render_config *rc, u32 *width, u32 *height, std::
                " contradicts render_resolution = " + std::to_string(res) + " (set it to 0)";
         return false;
     }
-    *width = w != 0 ? w : res;
-    *height = h != 0 ? h : res;
-    if ((uint64_t)*width * *height * 4 > 0xffffffffull) {
-        *err = "render image of " + std::to_string(*width) + " x " + std::to_string(*height) +
+    out->width = w != 0 ? w : res;
+    out->height = h != 0 ? h : res;
+    if ((uint64_t)out->width * out->height * 4 > 0xffffffffull) {
+        *err = "render image of " + std::to_string(out->width) + " x " + std::to_string(out->height) +
                " pixels: its 4-byte-per-pixel output buffers exceed the 32-bit component size";
         return false;
     }
-    return true;
-}
-
-// Whether a render config asks for the segmentation output (0 off, 1 on; else invalid).
-bool renderSegmentation(const mb2_render_config *rc, u32 *on, std::string *err)
-{
     if (rc->segmentation > 1) {
         *err = "segmentation = " + std::to_string(rc->segmentation) + " is not 0 (off) or 1 (on)";
         return false;
     }
-    *on = rc->segmentation;
-    return true;
-}
-
-// The camera model of a render config (0 pinhole, 1 panorama; else invalid).
-bool renderProjection(const mb2_render_config *rc, u32 *projection, std::string *err)
-{
+    out->segmentation = rc->segmentation;
     if (rc->projection > 1) {
         *err = "projection = " + std::to_string(rc->projection) + " is not 0 (pinhole) or 1 (panorama)";
         return false;
     }
-    *projection = rc->projection;
+    out->projection = rc->projection;
     return true;
 }
 
 bool renderHostCreate(Executor *ex, const mb2_render_config *rc, std::string *err)
 {
-    u32 width = 0, height = 0, segmentation = 0, projection = 0;
-    if (rc && (!renderImageSize(rc, &width, &height, err) || !renderSegmentation(rc, &segmentation, err) ||
-               !renderProjection(rc, &projection, err))) return false;
     RenderHost *rh = new RenderHost();
     ex->render = rh;
     memset(&rh->hRender, 0, sizeof(RenderState));
@@ -1720,18 +1707,19 @@ bool renderHostCreate(Executor *ex, const mb2_render_config *rc, std::string *er
     }
     ex->allocations.push_back(rh->dRender);
     RenderState &R = rh->hRender;
-    if (rc && width > 0) {
+    const RenderSettings &cfg = ex->renderSettings;
+    if (rc && cfg.width > 0) {
         if (!rc->geo_bvh_data.mesh_bvhs || rc->geo_bvh_data.num_bvhs == 0) {
             *err = "CudaBatchRenderConfig::geoBVHData is empty (build it with mb2_build_mesh_bvhs / "
                    "render::AssetProcessor::makeBVHData)";
             return false;
         }
         R.enabled = 1;
-        R.width = width;
-        R.height = height;
+        R.width = cfg.width;
+        R.height = cfg.height;
         R.rgbd = rc->render_mode == 0 ? 1u : 0u;
-        R.segmentation = segmentation;
-        R.projection = projection;
+        R.segmentation = cfg.segmentation;
+        R.projection = cfg.projection;
         R.nearPlane = rc->near_plane;
         R.farPlane = rc->far_plane;
         // device pointers, adopted as they are (the reference frees them in its
@@ -1741,8 +1729,7 @@ bool renderHostCreate(Executor *ex, const mb2_render_config *rc, std::string *er
         R.materials = (const RenderMaterial *)rc->material_data.materials;
         R.textures = (const unsigned long long *)rc->material_data.textures;
         R.numTextures = R.textures ? rc->material_data.num_texture_buffers : 0u;
-        const char *dbg = getenv("MADRONA_B200_RENDER_DEBUG");
-        R.debugHits = (dbg && *dbg && *dbg != '0') ? 1u : 0u;
+        R.debugHits = ex->knobs.renderDebug ? 1u : 0u;
     }
     cudaMemcpy(rh->dRender, &R, sizeof(RenderState), cudaMemcpyHostToDevice);
     ex->hState->render = rh->dRender;
