@@ -94,8 +94,15 @@ typedef struct mb2_material_view {
  * columns span azimuth -180..180 degrees (0 = the view's forward, columns turning
  * toward +u as the pinhole's do) and whose rows span the vertical field of view
  * evenly in elevation; depth is then the distance along the unit ray (a lidar's
- * range).  mb2_executor_create returns NULL and mb2_last_error() says why when any
- * of this does not hold (segmentation and projection are 0 or 1). */
+ * range).  normals = 1 (not in the reference) gives every view one more output,
+ * row-major [render_height][render_width] of int8 x, y, z, w: round(127 n) of the
+ * unit geometric normal n of the triangle the pixel's primary ray hits first
+ * (the hit of depth and segmentation), in the view's frame (+x toward increasing
+ * column, +y toward increasing row, +z away from the camera), turned to face the
+ * camera, w = 0; (0, 0, 0, 0) where the ray hits nothing, so exactly where the
+ * depth is 0; 0 (zero-initialised) leaves it out.  mb2_executor_create returns
+ * NULL and mb2_last_error() says why when any of this does not hold
+ * (segmentation, projection and normals are 0 or 1). */
 typedef struct mb2_render_config {
     uint32_t render_mode;          /* 0 RGBD, 1 Depth */
     mb2_mesh_bvh_view geo_bvh_data;
@@ -107,6 +114,7 @@ typedef struct mb2_render_config {
     uint32_t render_height;        /* rows per view, or 0 */
     uint32_t segmentation;         /* 1: per-pixel entity ids, 0: none */
     uint32_t projection;           /* 0 pinhole, 1 panorama */
+    uint32_t normals;              /* 1: per-pixel surface normals, 0: none */
 } mb2_render_config;
 
 /* Triangle mesh -> BLAS.  Role of MeshBVHBuilder (src/common/mesh_bvh_builder.cpp,

@@ -41,6 +41,7 @@ struct RenderSettings {
     uint32_t width = 0, height = 0;
     uint32_t segmentation = 0;   // 1: the per-pixel entity id output
     uint32_t projection = 0;     // 0 pinhole, 1 panorama
+    uint32_t normals = 0;        // 1: the per-pixel surface normal output
 };
 
 struct Executor {

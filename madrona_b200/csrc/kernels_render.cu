@@ -28,7 +28,8 @@
 // (reference-format MeshBVH: quantised 4-wide nodes over de-indexed triangles)
 // -> watertight ray / triangle test; materials (override colour / material
 // table, material textures sampled at the final hit's uv), lights with shadow
-// rays, RGBA8 + f32 depth (+ the hit entity's id when the config asks for segmentation).
+// rays, RGBA8 + f32 depth (+ the hit entity's id when the config asks for segmentation,
+// + the hit triangle's int8 normal when it asks for normals).
 // Views are pinholes, or with projection = 1 360-degree equirectangular panoramas.
 //
 // Image formation follows the reference's CUDA ray tracer
@@ -1265,6 +1266,36 @@ __device__ __forceinline__ bool boxOutside(const float *lo, const float *hi, Vec
     return reach < 0.f;
 }
 
+// ---- surface normals (mb2_render_config::normals = 1) ------------------------------------------
+// The geometric normal of a hit triangle (object-space vertices tv, world -> object linear part
+// m of its instance) as int8 x, y, z, w = 0 packed in a word: round(127 n) with n the unit
+// normal in the view's frame (x = n.u, y = n.vv, z = n.forward), turned against the ray.
+// M^T (b - a) x (c - a) is the cross product of the world-space edges up to the sign of det M,
+// so non-uniform and mirroring scales give the true surface normal; the orientation removes
+// the sign.  A hit never encodes to 0 (some component of a unit vector is >= 1/sqrt 3); a
+// triangle with a zero cross product does, as a miss does.
+__device__ __forceinline__ u32 encodeHitNormal(const BVHVertex *tv, const float *m, Vector3 ray_dir,
+                                               Vector3 u, Vector3 vv, Vector3 forward)
+{
+    const Vector3 a { tv[0].pos[0], tv[0].pos[1], tv[0].pos[2] };
+    const Vector3 b { tv[1].pos[0], tv[1].pos[1], tv[1].pos[2] };
+    const Vector3 c { tv[2].pos[0], tv[2].pos[1], tv[2].pos[2] };
+    const Vector3 no = cross(b - a, c - a);
+    const Vector3 n { m[0] * no.x + m[3] * no.y + m[6] * no.z,
+                      m[1] * no.x + m[4] * no.y + m[7] * no.z,
+                      m[2] * no.x + m[5] * no.y + m[8] * no.z };
+    const float s = dot(n, ray_dir) > 0.f ? -1.f : 1.f;
+    float x = s * dot(n, u), y = s * dot(n, vv), z = s * dot(n, forward);
+    // scaled to a largest component of 1 first: tiny and huge triangles keep their direction
+    const float big = fmaxf(fabsf(x), fmaxf(fabsf(y), fabsf(z)));
+    if (!(big > 0.f && big < INFINITY)) return 0u;
+    const float r = __frcp_rn(big);
+    x *= r; y *= r; z *= r;
+    const float k = 127.f * rsqrtf(x * x + y * y + z * z);
+    auto q = [](float v) { return (u32)min(max(__float2int_rn(v), -127), 127) & 0xffu; };
+    return q(k * x) | (q(k * y) << 8) | (q(k * z) << 16);
+}
+
 // ---- panoramas (mb2_render_config::projection = 1) ---------------------------------------------
 // Pixel (px, py) of a W x H panorama looks at azimuth theta = s 2 pi ((px + 0.5) / W - 0.5) and
 // elevation phi = 2 phi_max ((py + 0.5) / H - 0.5), phi_max = atan(h) and s = sign(h), in the
@@ -1317,7 +1348,10 @@ constexpr int kRaycastMinBlocks = 3;   // blocks per SM the ray caster is compil
 // MATERIALS: the render config has a material table.  Without one no hit can name a texture,
 // so the texture code is left out and such scenes keep the code they had before textures.
 // PANORAMA: the render config's projection is the 360-degree panorama (else the pinhole).
-template <bool FLAT, bool MATERIALS, bool PANORAMA>
+// NORMALS: the render config asks for the surface normal output.  A template parameter, not a
+// runtime branch: the normal's vertex loads and matrix stay out of the other instantiations,
+// which keep their registers, stack and spills.
+template <bool FLAT, bool MATERIALS, bool PANORAMA, bool NORMALS>
 __global__ void __launch_bounds__(256, kRaycastMinBlocks)
 renderRaycastKernel(EngineState *Sp)
 {
@@ -1541,6 +1575,17 @@ renderRaycastKernel(EngineState *Sp)
                 i32 *seg_out = (i32 *)((char *)out_tbl.columns[R.segCol] + off);
                 *seg_out = hit ? instances[first.instance].entityID : -1;
             }
+            if (NORMALS) {
+                // the same closest hit again: all zero exactly where the depth is 0
+                u32 nrm = 0;
+                if (hit) {
+                    const RenderInstance &inst = instances[first.instance];
+                    const InstanceXform X = instanceXform(inst);
+                    nrm = encodeHitNormal(R.meshes[inst.objectID].vertices + (size_t)first.triangle * 3, X.m,
+                                          ray_dir, u, vv, forward);
+                }
+                *(u32 *)((char *)out_tbl.columns[R.normalCol] + off) = nrm;
+            }
             if (R.hitIDs) {
                 i32 *ids = R.hitIDs + ((size_t)view.outputRow * pixels_per_view + pix) * 2;
                 ids[0] = hit ? first.instance : -1;
@@ -1661,7 +1706,7 @@ static std::vector<LightCarrierArchetype> &lightCarriers(Executor *ex)
 }
 
 // The image is render_width x render_height when both are set, else the render_resolution
-// square; segmentation and projection are 0 or 1.
+// square; segmentation, projection and normals are 0 or 1.
 bool renderParseConfig(const mb2_render_config *rc, RenderSettings *out, std::string *err)
 {
     *out = RenderSettings();
@@ -1693,6 +1738,11 @@ bool renderParseConfig(const mb2_render_config *rc, RenderSettings *out, std::st
         return false;
     }
     out->projection = rc->projection;
+    if (rc->normals > 1) {
+        *err = "normals = " + std::to_string(rc->normals) + " is not 0 (off) or 1 (on)";
+        return false;
+    }
+    out->normals = rc->normals;
     return true;
 }
 
@@ -1720,6 +1770,7 @@ bool renderHostCreate(Executor *ex, const mb2_render_config *rc, std::string *er
         R.rgbd = rc->render_mode == 0 ? 1u : 0u;
         R.segmentation = cfg.segmentation;
         R.projection = cfg.projection;
+        R.normals = cfg.normals;
         R.nearPlane = rc->near_plane;
         R.farPlane = rc->far_plane;
         // device pointers, adopted as they are (the reference frees them in its
@@ -1788,6 +1839,7 @@ bool renderHostAfterRegistry(Executor *ex, std::string *err)
     R.rgbCol = col(R.outputArchetype, R.cidRGB);
     R.depthCol = col(R.outputArchetype, R.cidDepth);
     R.segCol = col(R.outputArchetype, R.cidSegmentation);
+    R.normalCol = col(R.outputArchetype, R.cidNormal);
     R.lightCol = col(R.lightArchetype, R.cidLightDesc);
     // the output table may grow (during world construction or between steps): the view
     // list covers every row it can ever have, so no view is left unrendered
@@ -1957,6 +2009,19 @@ void *renderDebugBuffer(Executor *ex, int which)
     }
 }
 
+// the flat-list and the TLAS instantiation of the ray caster, on the executor's stream
+template <bool MATERIALS, bool PANORAMA>
+static void launchRaycastPair(Executor *ex, unsigned view_blocks, u32 normals)
+{
+    if (normals) {
+        renderRaycastKernel<true, MATERIALS, PANORAMA, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+        renderRaycastKernel<false, MATERIALS, PANORAMA, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+    } else {
+        renderRaycastKernel<true, MATERIALS, PANORAMA, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+        renderRaycastKernel<false, MATERIALS, PANORAMA, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+    }
+}
+
 LaunchGraph *physicsBuildRenderGraph(Executor *ex, std::string *err)
 {
     RenderHost *rh = ex->render;
@@ -1980,19 +2045,12 @@ LaunchGraph *physicsBuildRenderGraph(Executor *ex, std::string *err)
     // 1024 worlds); 8 rounds of resident blocks keep the tail short
     const unsigned view_blocks = (unsigned)std::max(1, std::min(R.maxViews, ex->numSMs * kRaycastMinBlocks * 8));
     if (R.projection == 1) {
-        if (R.materials) {
-            renderRaycastKernel<true, true, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
-            renderRaycastKernel<false, true, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
-        } else {
-            renderRaycastKernel<true, false, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
-            renderRaycastKernel<false, false, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
-        }
+        if (R.materials) launchRaycastPair<true, true>(ex, view_blocks, R.normals);
+        else launchRaycastPair<false, true>(ex, view_blocks, R.normals);
     } else if (R.materials) {
-        renderRaycastKernel<true, true, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
-        renderRaycastKernel<false, true, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+        launchRaycastPair<true, false>(ex, view_blocks, R.normals);
     } else {
-        renderRaycastKernel<true, false, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
-        renderRaycastKernel<false, false, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+        launchRaycastPair<false, false>(ex, view_blocks, R.normals);
     }
     launchStatusCopy(ex, ex->stream);
     cudaError_t e = cudaStreamEndCapture(ex->stream, &g->graph);
@@ -2007,13 +2065,14 @@ LaunchGraph *physicsBuildRenderGraph(Executor *ex, std::string *err)
 }
 
 // algorithmic bytes of one frame (SURVEY.md 8d): W x H x 4 B depth (+ 4 B RGBA8)
-// (+ 4 B segmentation) per view
+// (+ 4 B segmentation) (+ 4 B normal) per view
 uint64_t renderBytesPerFrame(Executor *ex, int64_t num_views)
 {
     RenderHost *rh = ex->render;
     if (!rh || !rh->active) return 0;
     const RenderState &R = rh->hRender;
-    return (uint64_t)num_views * R.width * R.height * (4ull + (R.rgbd ? 4ull : 0ull) + (R.segmentation ? 4ull : 0ull));
+    return (uint64_t)num_views * R.width * R.height *
+        (4ull + (R.rgbd ? 4ull : 0ull) + (R.segmentation ? 4ull : 0ull) + (R.normals ? 4ull : 0ull));
 }
 
 }

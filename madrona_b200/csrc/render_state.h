@@ -88,6 +88,7 @@ struct RenderState {
     u32 debugHits;                  // MADRONA_B200_RENDER_DEBUG: keep (instance, triangle) per pixel
     u32 segmentation;               // 1: each view also gets an i32 entity id per pixel
     u32 projection;                 // 0: pinhole, 1: 360-degree equirectangular panorama
+    u32 normals;                    // 1: each view also gets an int8 x 4 surface normal per pixel
 
     // ---- written by the device-side RenderingSystem::registerTypes
     u32 registered;
@@ -95,14 +96,14 @@ struct RenderState {
     u32 lightArchetype, cidLightDesc;
     u32 cidPosition, cidRotation, cidScale, cidObjectID;
     u32 outputArchetype;   // RaycastOutputArchetype
-    u32 cidRGB, cidDepth, cidSegmentation;
+    u32 cidRGB, cidDepth, cidSegmentation, cidNormal;
 
     // ---- filled by the host after registerTypes
     u32 numRenderArchetypes;
     RenderArchetype renderables[kMaxRenderArchetypes];
     u32 numViewArchetypes;
     ViewArchetype viewers[kMaxRenderArchetypes];
-    i32 rgbCol, depthCol, segCol;
+    i32 rgbCol, depthCol, segCol, normalCol;
 
     // Instances are one world-major list: world w's, in gather order, start at
     // instanceOffsets[w] (exclusive scan of instanceCounts).  The list, the TLAS nodes and

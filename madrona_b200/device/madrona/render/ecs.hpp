@@ -75,11 +75,16 @@ struct DepthOutputBuffer : RenderOutputBuffer {};
 // Not in the reference: height x width i32 per view, the Entity::id of the renderable each
 // pixel's primary ray hits first, -1 where it hits nothing (mb2_render_config::segmentation)
 struct SegmentationOutputBuffer : RenderOutputBuffer {};
+// Not in the reference: height x width int8 x 4 per view, the camera-facing unit normal of the
+// triangle each pixel's primary ray hits first in the view's frame, x 127, w = 0; all zero where
+// it hits nothing (mb2_render_config::normals)
+struct NormalOutputBuffer : RenderOutputBuffer {};
 
 struct RaycastOutputArchetype : public Archetype<
     RGBOutputBuffer,
     DepthOutputBuffer,
-    SegmentationOutputBuffer
+    SegmentationOutputBuffer,
+    NormalOutputBuffer
 > {};
 
 struct RenderECSBridge;
@@ -112,6 +117,8 @@ inline void registerTypes(ECSRegistry &registry, const RenderECSBridge *)
     registry.registerComponent<DepthOutputBuffer>(bytes);
     // a view row carries 4 bytes of it when segmentation is off
     registry.registerComponent<SegmentationOutputBuffer>(R.segmentation ? bytes : 4u);
+    // and of this one when normals are off
+    registry.registerComponent<NormalOutputBuffer>(R.normals ? bytes : 4u);
     registry.registerArchetype<RaycastOutputArchetype>();
     registry.registerArchetype<LightArchetype>();
 
@@ -129,6 +136,7 @@ inline void registerTypes(ECSRegistry &registry, const RenderECSBridge *)
     R.cidRGB = TypeTracker::typeID<RGBOutputBuffer>();
     R.cidDepth = TypeTracker::typeID<DepthOutputBuffer>();
     R.cidSegmentation = TypeTracker::typeID<SegmentationOutputBuffer>();
+    R.cidNormal = TypeTracker::typeID<NormalOutputBuffer>();
     R.registered = 1;
 }
 

@@ -117,7 +117,7 @@ class _MaterialViewC(ctypes.Structure):      # == render::MaterialData
     ]
 
 
-class _RenderConfigC(ctypes.Structure):      # == madrona::CudaBatchRenderConfig + image size + outputs + projection
+class _RenderConfigC(ctypes.Structure):      # == madrona::CudaBatchRenderConfig + image size + outputs + projection + normals
     _fields_ = [
         ("render_mode", ctypes.c_uint32),
         ("geo_bvh_data", _MeshBVHViewC),
@@ -132,6 +132,9 @@ class _RenderConfigC(ctypes.Structure):      # == madrona::CudaBatchRenderConfig
         ("segmentation", ctypes.c_uint32),
         # camera model of every view: 0 pinhole, 1 360-degree equirectangular panorama
         ("projection", ctypes.c_uint32),
+        # 1: per view one more output, int8 [height][width][4]: the hit triangle's camera-facing
+        # normal x 127 in the view's frame (w = 0), all zero on a miss
+        ("normals", ctypes.c_uint32),
     ]
 
 

@@ -156,8 +156,14 @@ struct RenderImageSize {
 // (without its generation) of the renderable each pixel's primary ray hits first, -1 where
 // it hits nothing.  Exported like the other outputs, through
 // exportColumn<render::RaycastOutputArchetype, render::SegmentationOutputBuffer>.
+// normals: every view also gets a row-major [height][width] image of int8 x, y, z, w, the
+// unit geometric normal of the hit triangle times 127 in the view's frame (+x toward increasing
+// column, +y toward increasing row, +z away from the camera), turned to face the camera, w = 0;
+// all zero where the ray hits nothing.  Exported through
+// exportColumn<render::RaycastOutputArchetype, render::NormalOutputBuffer>.
 struct RenderOutputs {
     bool segmentation;
+    bool normals;
 };
 
 // The camera model of every view, for the MWCudaExecutor constructor overload that takes one.
@@ -392,6 +398,7 @@ private:
             rc.render_width = image_size.width;
             rc.render_height = image_size.height;
             rc.segmentation = outputs.segmentation ? 1u : 0u;
+            rc.normals = outputs.normals ? 1u : 0u;
             rc.projection = (uint32_t)projection;
         }
         int gpu_id = mb2_device_of_context((void *)cu_ctx);

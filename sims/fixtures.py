@@ -147,10 +147,11 @@ def _image_size(cfg, default_res):
 
 def _render_options(cfg, default_res):
     """Keyword arguments for the render_assets builders: the image size, `segmentation`
-    (per-pixel hit entity ids) and `panorama` (360-degree equirectangular views instead of
-    pinholes), both off unless the fixture config sets them."""
+    (per-pixel hit entity ids), `panorama` (360-degree equirectangular views instead of
+    pinholes) and `normals` (per-pixel surface normals), all off unless the fixture config sets
+    them."""
     return dict(_image_size(cfg, default_res), segmentation=bool(cfg.get("segmentation", False)),
-                panorama=bool(cfg.get("panorama", False)))
+                panorama=bool(cfg.get("panorama", False)), normals=bool(cfg.get("normals", False)))
 
 
 def _room_render_cfg(cfg):
@@ -333,11 +334,12 @@ SIMS: Dict[str, SimDesc] = {
     "hullpile_big_many": _hullpile_desc("hullpile_big_many", 60, ["-DHULLPILE_MANY=1"],
                                         objects=_hullpile_big_objects),
     # GPU only: batch ray caster with a real TLAS / BLAS, materials, lights (tests/test_render_bvh.py);
-    # -DGALLERY_ENTITY_EXPORTS=1 adds the props' entities and the segmentation output (slots 10, 11)
+    # -DGALLERY_ENTITY_EXPORTS=1 adds the props' entities and the segmentation output (slots 10, 11),
+    # -DGALLERY_NORMAL_EXPORTS=1 the surface normal output (slot 12)
     "gallery": SimDesc(
         name="gallery",
         sources=[os.path.join(_ROOT, "gallery", "sim.cpp")],
-        num_exports=12,
+        num_exports=13,
         num_taskgraphs=1,
         inputs=[],
         outputs=[],
@@ -345,7 +347,7 @@ SIMS: Dict[str, SimDesc] = {
         pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
         oracle_extra=lambda cfg: [],
         defaults={"num_props": 100, "seed": 0, "resolution": 40, "rgbd": True},
-        compile_flags=["-DGALLERY_ENTITY_EXPORTS=1"],
+        compile_flags=["-DGALLERY_ENTITY_EXPORTS=1", "-DGALLERY_NORMAL_EXPORTS=1"],
         render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_render_config(
             rgbd=bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)), **_render_options(cfg, 40)),
     ),
@@ -354,7 +356,7 @@ SIMS: Dict[str, SimDesc] = {
     "gallery_sized": SimDesc(
         name="gallery_sized",
         sources=[os.path.join(_ROOT, "gallery", "sim.cpp")],
-        num_exports=12,
+        num_exports=13,
         num_taskgraphs=1,
         inputs=[],
         outputs=[],
@@ -363,7 +365,7 @@ SIMS: Dict[str, SimDesc] = {
                                              int(cfg["layouts"][w]) if cfg.get("layouts") else 0),
         oracle_extra=lambda cfg: [],
         defaults={"props": [100], "layouts": None, "seed": 0, "resolution": 40, "rgbd": True},
-        compile_flags=["-DGALLERY_PER_WORLD=1", "-DGALLERY_ENTITY_EXPORTS=1"],
+        compile_flags=["-DGALLERY_PER_WORLD=1", "-DGALLERY_ENTITY_EXPORTS=1", "-DGALLERY_NORMAL_EXPORTS=1"],
         render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_render_config(
             rgbd=bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)), **_render_options(cfg, 40)),
     ),
@@ -372,7 +374,7 @@ SIMS: Dict[str, SimDesc] = {
     "gallery_textured": SimDesc(
         name="gallery_textured",
         sources=[os.path.join(_ROOT, "gallery", "sim.cpp")],
-        num_exports=12,
+        num_exports=13,
         num_taskgraphs=1,
         inputs=[],
         outputs=[],
@@ -380,7 +382,7 @@ SIMS: Dict[str, SimDesc] = {
         pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
         oracle_extra=lambda cfg: [],
         defaults={"num_props": 100, "seed": 0, "resolution": 40, "rgbd": True, "bc7": False},
-        compile_flags=["-DGALLERY_ENTITY_EXPORTS=1"],
+        compile_flags=["-DGALLERY_ENTITY_EXPORTS=1", "-DGALLERY_NORMAL_EXPORTS=1"],
         render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_textured_render_config(
             rgbd=bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)),
             bc7=bool(cfg.get("bc7", False)), **_render_options(cfg, 40)),

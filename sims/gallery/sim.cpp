@@ -29,6 +29,9 @@ void Sim::registerTypes(ECSRegistry &registry, const Config &)
 #if defined(GALLERY_ENTITY_EXPORTS)
     registry.exportColumn<Prop, Entity>((uint32_t)ExportID::PropEntity);
     registry.exportColumn<RaycastOutputArchetype, SegmentationOutputBuffer>((uint32_t)ExportID::Segmentation);
+#if defined(GALLERY_NORMAL_EXPORTS)
+    registry.exportColumn<RaycastOutputArchetype, NormalOutputBuffer>((uint32_t)ExportID::Normals);
+#endif
 #endif
 }
 

@@ -26,13 +26,15 @@ using madrona::base::ObjectID;
 constexpr int32_t kNumViews = 2;
 constexpr int32_t kNumLights = 2;
 
-// PropEntity and Segmentation are exported when built with -DGALLERY_ENTITY_EXPORTS=1 (as the
-// fixtures are); without it the gallery exports the first ten slots only
+// PropEntity and Segmentation are exported when built with -DGALLERY_ENTITY_EXPORTS=1, Normals
+// when also built with -DGALLERY_NORMAL_EXPORTS=1 (as the fixtures are); without them the
+// gallery exports the first ten (or twelve) slots only
 enum class ExportID : uint32_t {
     PropPos, PropRot, PropScale, PropObj, PropMat, PropColor,
     ViewPos, ViewRot,
     RGB, Depth,
     PropEntity, Segmentation,
+    Normals,
     NumExports,
 };
 

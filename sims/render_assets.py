@@ -49,12 +49,13 @@ def mesh_list(descs, verts, indices):
 
 def make_render_config_from_meshes(meshes, resolution: int, rgbd: bool, gpu_id: int = 0, materials=None,
                                    width: int = 0, height: int = 0, segmentation: bool = False,
-                                   panorama: bool = False):
+                                   panorama: bool = False, normals: bool = False):
     """mb2_render_config (== CudaBatchRenderConfig) whose geoBVHData was built by the
     engine's BLAS builder; returns (config, keep_alive).  width x height images when both are
     given (resolution then 0 or equal to both), else resolution squared.  segmentation: every
     view also gets an int32 image of hit entity ids.  panorama: every view is a 360-degree
-    equirectangular panorama instead of a pinhole."""
+    equirectangular panorama instead of a pinhole.  normals: every view also gets an int8 x 4
+    image of the hit triangles' camera-facing normals in the view's frame."""
     import madrona_b200 as mb
     from madrona_b200.executor import _MaterialViewC, _RenderConfigC
 
@@ -67,16 +68,16 @@ def make_render_config_from_meshes(meshes, resolution: int, rgbd: bool, gpu_id: 
         keep.append(m)
         mat_view = _MaterialViewC(None, 0, None, m.data_ptr())
     rc = _RenderConfigC(0 if rgbd else 1, bvh.view(device=True), mat_view, resolution, 0.001, 1000.0,
-                        width, height, int(segmentation), int(panorama))
+                        width, height, int(segmentation), int(panorama), int(normals))
     return rc, keep
 
 
 def make_render_config(resolution: int, rgbd: bool = False, gpu_id: int = 0, width: int = 0, height: int = 0,
-                       segmentation: bool = False, panorama: bool = False):
+                       segmentation: bool = False, panorama: bool = False, normals: bool = False):
     descs, verts, indices = room_meshes()
     return make_render_config_from_meshes(mesh_list(descs, verts, indices), resolution, rgbd, gpu_id,
                                           width=width, height=height, segmentation=segmentation,
-                                          panorama=panorama)
+                                          panorama=panorama, normals=normals)
 
 
 # ---- gallery fixture: four prop meshes + ground ------------------------------------------------
@@ -143,10 +144,10 @@ GALLERY_MATERIALS[:, 4] = np.array([-1], dtype=np.int32).view(np.float32)[0]    
 
 
 def make_gallery_render_config(resolution: int, rgbd: bool, gpu_id: int = 0, width: int = 0, height: int = 0,
-                               segmentation: bool = False, panorama: bool = False):
+                               segmentation: bool = False, panorama: bool = False, normals: bool = False):
     return make_render_config_from_meshes(gallery_meshes(), resolution, rgbd, gpu_id, materials=GALLERY_MATERIALS,
                                           width=width, height=height, segmentation=segmentation,
-                                          panorama=panorama)
+                                          panorama=panorama, normals=normals)
 
 
 # ---- textured gallery: the same meshes with uvs, three generated textures -----------------------
@@ -295,7 +296,7 @@ def gallery_textured_materials(bc7: bool = False):
 
 def make_gallery_textured_render_config(resolution: int, rgbd: bool, gpu_id: int = 0, bc7: bool = False,
                                         width: int = 0, height: int = 0, segmentation: bool = False,
-                                        panorama: bool = False):
+                                        panorama: bool = False, normals: bool = False):
     """CudaBatchRenderConfig with textured materials uploaded by mb2_init_material_data; the
     MaterialData in keep_alive must outlive the executor."""
     import madrona_b200 as mb
@@ -305,5 +306,5 @@ def make_gallery_textured_render_config(resolution: int, rgbd: bool, gpu_id: int
     textures = [(src, fmt, t.shape[1], t.shape[0]) for t, fmt, src in gallery_textures()]
     mats = mb.MaterialData(gallery_textured_materials(bc7), textures, gpu_id=gpu_id)
     rc = _RenderConfigC(0 if rgbd else 1, bvh.view(device=True), mats.view(), resolution, 0.001, 1000.0,
-                        width, height, int(segmentation), int(panorama))
+                        width, height, int(segmentation), int(panorama), int(normals))
     return rc, [bvh, mats]
