@@ -252,6 +252,59 @@ void *mb2_render_debug_hits(mb2_executor *exec);
  * no per-world stride).  Device pointers; NULL without a renderer. */
 void *mb2_render_debug_buffer(mb2_executor *exec, int which, int64_t *stride);
 
+/* ---- free views of the ray caster -------------------------------------------
+ * No reference counterpart.  Ray-casts caller-given views of the scene the last
+ * render-prepare built (the state after the last step: instances, lights,
+ * shadows, textures, material and colour overrides, hidden renderables) into
+ * caller-owned device buffers.  Changes made since that prepare are not seen;
+ * before the first prepare every pixel is a miss; after a snapshot restore the
+ * saved scene is rendered.  The ECS tables, the exported render outputs and the
+ * simulation state are not touched.
+ *   - A view is what a camera entity gives the renderer: world; position, the
+ *     camera's world position (entity position plus camera offset); rotation,
+ *     the viewing entity's Rotation (w, x, y, z; the camera looks along the
+ *     rotated +y, +x is to its right); vfov_degrees, the vertical field of view
+ *     as attachEntityToView takes it.  A view with the pose, field of view,
+ *     image size and projection of one of the simulator's cameras writes the
+ *     render graph's bytes for that camera (with the simulator compiled without
+ *     FMA contraction, MADRONA_B200_FAST_MATH=0, the default).
+ *   - Every view of a call is width x height pixels (each >= 1, width * height
+ *     * 4 within 32 bits) and has one projection: 0 pinhole, 1 panorama (see
+ *     mb2_render_config).  The same world may appear any number of times, in any
+ *     order.
+ *   - outputs: device pointers or NULL, in the layouts of the exported columns,
+ *     view i at slice i: rgb uint8 [n][H][W][4], depth float32 [n][H][W],
+ *     segmentation int32 [n][H][W], normals int8 [n][H][W][4].  None depends on
+ *     the executor's config: a depth-only executor, or one without
+ *     segmentation, normals or panoramas, writes all of them here.
+ *   - Enqueued on cuda_stream (NULL: the executor's stream), never synchronizing
+ *     the host; the views are copied before the call returns.  It reads the
+ *     prepared scene, which the step graph's render-prepare rewrites, so it is
+ *     part of the "one launch graph in flight" rule: put it on the stream of the
+ *     steps or chain the streams with events.  Device-side errors (a material's
+ *     texture index past the config) are published like the render graph's and
+ *     fail the next mb2_run.
+ *   - Returns 0, or 1 with a message in mb2_last_error() and nothing launched
+ *     for: a null executor or views, num_views == 0, an executor without a
+ *     renderer, a world outside [0, num_worlds), a non-finite position, rotation
+ *     or field of view, vfov_degrees outside (0, 180), an image size outside the
+ *     rules, projection not 0 or 1, or all four outputs NULL. */
+typedef struct mb2_free_view {
+    int32_t world;
+    float position[3];
+    float rotation[4];             /* w, x, y, z */
+    float vfov_degrees;
+} mb2_free_view;
+typedef struct mb2_free_view_outputs {
+    void *rgb;
+    void *depth;
+    void *segmentation;
+    void *normals;
+} mb2_free_view_outputs;
+int mb2_render_free_views(mb2_executor *exec, const mb2_free_view *views, uint32_t num_views,
+                          uint32_t width, uint32_t height, uint32_t projection,
+                          const mb2_free_view_outputs *outputs, void *cuda_stream);
+
 /* Kernel nodes inside a built launch graph (== launches per run). */
 int64_t mb2_launch_graph_num_kernels(const mb2_launch_graph *graph);
 

@@ -1347,6 +1347,26 @@ void *mb2_render_debug_buffer(mb2_executor *exec, int which, int64_t *stride)
     return exec ? renderDebugBuffer((Executor *)exec, which) : nullptr;
 }
 
+int mb2_render_free_views(mb2_executor *exec, const mb2_free_view *views, uint32_t num_views, uint32_t width,
+                          uint32_t height, uint32_t projection, const mb2_free_view_outputs *outputs,
+                          void *cuda_stream)
+{
+    g_last_error.clear();
+    if (!exec || !views) {
+        setError("mb2_render_free_views: null executor or views");
+        return 1;
+    }
+    Executor *ex = (Executor *)exec;
+    const mb2_free_view_outputs out = outputs ? *outputs : mb2_free_view_outputs {};
+    std::string err;
+    if (!renderFreeViews(ex, views, num_views, width, height, projection, out,
+                         cuda_stream ? (cudaStream_t)cuda_stream : ex->stream, &err)) {
+        setError("mb2_render_free_views: " + err);
+        return 1;
+    }
+    return 0;
+}
+
 int64_t mb2_launch_graph_num_branches(const mb2_launch_graph *graph)
 {
     return graph ? ((const LaunchGraph *)graph)->numBranches : -1;

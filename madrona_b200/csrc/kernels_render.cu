@@ -24,7 +24,8 @@
 //   centres inside the world's bounds, Karras' parallel LBVH, bottom-up boxes, collapse to
 //   4-wide nodes, quantise -> QBVHNode[] (the reference's traversal format)
 // Render graph: renderRaycastKernel, one thread per pixel, one block per view
-// (8 x 4 pixel tiles per warp): TLAS -> instance -> object-space ray -> BLAS
+// (8 x 4 pixel tiles per warp; free views, renderFreeViews, split a view's tiles over
+// blocks): TLAS -> instance -> object-space ray -> BLAS
 // (reference-format MeshBVH: quantised 4-wide nodes over de-indexed triangles)
 // -> watertight ray / triangle test; materials (override colour / material
 // table, material textures sampled at the final hit's uv), lights with shadow
@@ -52,6 +53,7 @@
 
 #include <madrona/math.hpp>
 #include <cfloat>
+#include <cmath>
 #include <algorithm>
 #include <vector>
 
@@ -70,6 +72,9 @@ struct RenderHost {
     bool active = false;
     // instance list, TLAS nodes, large-world key / node scratch: one entry per renderable row
     VMRange instanceRange, nodeRange, keyRange, buildRange;
+    // free views (renderFreeViews): [freeViewCapacity] RenderView, then as many mb2_free_view
+    char *freeViews = nullptr;
+    u32 freeViewCapacity = 0;
 };
 
 // scratch entry of renderBuildLargeTLASKernel, one per instance of the world
@@ -1351,15 +1356,23 @@ constexpr int kRaycastMinBlocks = 3;   // blocks per SM the ray caster is compil
 // NORMALS: the render config asks for the surface normal output.  A template parameter, not a
 // runtime branch: the normal's vertex loads and matrix stay out of the other instantiations,
 // which keep their registers, stack and spills.
-template <bool FLAT, bool MATERIALS, bool PANORAMA, bool NORMALS>
+// FREE: the launch traces free views (renderFreeViews): `job` names the views, their size and
+// outputs, view i writes slice i, and the tiles of a view are split over blockIdx.x (block x
+// takes tiles x * warps + warp, stepping by gridDim.x * warps, and stages the flat instance
+// list itself).  Else the render graph's: views, size and output columns from RenderState and
+// the output table, one block per view.  A template parameter, not a runtime branch on `job`:
+// as a branch, its per-pixel selects cost the render graph 8 % on the flat path, while the
+// FREE = false instantiations compile to the code they had before free views.
+template <bool FLAT, bool MATERIALS, bool PANORAMA, bool NORMALS, bool FREE>
 __global__ void __launch_bounds__(256, kRaycastMinBlocks)
-renderRaycastKernel(EngineState *Sp)
+renderRaycastKernel(EngineState *Sp, const RaycastViews job)
 {
     EngineState &S = *Sp;
     const RenderState &R = *S.render;
     const TableDesc &out_tbl = S.tables[R.outputArchetype];
-    const i32 num_views = min(out_tbl.numRows, R.maxViews);
-    const u32 W = R.width, H = R.height;
+    constexpr bool graph = !FREE;
+    const i32 num_views = graph ? min(out_tbl.numRows, R.maxViews) : (i32)job.numViews;
+    const u32 W = graph ? R.width : job.width, H = graph ? R.height : job.height;
     // width / height of the image plane: exactly 1.0f for square images, whose planes and
     // rays therefore round as they did before images could be non-square
     const float aspect = (float)W / (float)H;
@@ -1381,7 +1394,7 @@ renderRaycastKernel(EngineState *Sp)
     __shared__ PanoCone s_cone[PANORAMA ? kFlatInstances : 1];     // s_list's cones (panoramas)
 
     for (i32 v = blockIdx.y; v < num_views; v += gridDim.y) {
-        const RenderView view = R.views[v];
+        const RenderView view = FREE ? job.views[v] : R.views[v];
         const i32 w = view.worldIDX;
         const i32 instance_offset = R.instanceOffsets[w];
         const QBVHNode *tlas = R.tlasNodes + instance_offset;
@@ -1478,7 +1491,9 @@ renderRaycastKernel(EngineState *Sp)
             }
         }
 
-        for (u32 tile = threadIdx.x >> 5; tile < num_tiles; tile += blockDim.x >> 5) {
+        const u32 warps = blockDim.x >> 5;
+        const u32 chunk = FREE ? blockIdx.x : 0u, chunks = FREE ? gridDim.x : 1u;
+        for (u32 tile = chunk * warps + (threadIdx.x >> 5); tile < num_tiles; tile += chunks * warps) {
             const u32 tx0 = (tile % tiles_x) * tile_w, ty0 = (tile / tiles_x) * tile_h;
             const u32 px = tx0 + (lane & (tile_w - 1));
             const u32 py = ty0 + (lane >> tile_shift);
@@ -1567,33 +1582,43 @@ renderRaycastKernel(EngineState *Sp)
             const bool hit = first.instance >= 0;
 
             const size_t pix = (size_t)px + (size_t)py * W;
-            const size_t off = (size_t)view.outputRow * bytes_per_view + 4 * pix;
-            float *depth_out = (float *)((char *)out_tbl.columns[R.depthCol] + off);
-            *depth_out = hit ? first.t : 0.f;
-            if (R.segmentation) {
-                // the same closest hit as the depth: -1 exactly where the depth is 0
-                i32 *seg_out = (i32 *)((char *)out_tbl.columns[R.segCol] + off);
-                *seg_out = hit ? instances[first.instance].entityID : -1;
-            }
-            if (NORMALS) {
-                // the same closest hit again: all zero exactly where the depth is 0
-                u32 nrm = 0;
-                if (hit) {
-                    const RenderInstance &inst = instances[first.instance];
-                    const InstanceXform X = instanceXform(inst);
-                    nrm = encodeHitNormal(R.meshes[inst.objectID].vertices + (size_t)first.triangle * 3, X.m,
-                                          ray_dir, u, vv, forward);
+            // the same closest hit again: all zero exactly where the depth is 0
+            auto hit_normal = [&]() -> u32 {
+                if (!hit) return 0;
+                const RenderInstance &inst = instances[first.instance];
+                const InstanceXform X = instanceXform(inst);
+                return encodeHitNormal(R.meshes[inst.objectID].vertices + (size_t)first.triangle * 3, X.m,
+                                       ray_dir, u, vv, forward);
+            };
+            unsigned char *rgb;
+            if (FREE) {
+                // view i writes slice i of every output the call asked for
+                const size_t off = (size_t)v * bytes_per_view + 4 * pix;
+                if (job.depth) *(float *)((char *)job.depth + off) = hit ? first.t : 0.f;
+                if (job.segmentation) {
+                    *(i32 *)((char *)job.segmentation + off) = hit ? instances[first.instance].entityID : -1;
                 }
-                *(u32 *)((char *)out_tbl.columns[R.normalCol] + off) = nrm;
+                if (NORMALS) *(u32 *)((char *)job.normals + off) = hit_normal();
+                if (!job.rgb) continue;
+                rgb = job.rgb + off;
+            } else {
+                const size_t off = (size_t)view.outputRow * bytes_per_view + 4 * pix;
+                float *depth_out = (float *)((char *)out_tbl.columns[R.depthCol] + off);
+                *depth_out = hit ? first.t : 0.f;
+                if (R.segmentation) {
+                    // the same closest hit as the depth: -1 exactly where the depth is 0
+                    i32 *seg_out = (i32 *)((char *)out_tbl.columns[R.segCol] + off);
+                    *seg_out = hit ? instances[first.instance].entityID : -1;
+                }
+                if (NORMALS) *(u32 *)((char *)out_tbl.columns[R.normalCol] + off) = hit_normal();
+                if (R.hitIDs) {
+                    i32 *ids = R.hitIDs + ((size_t)view.outputRow * pixels_per_view + pix) * 2;
+                    ids[0] = hit ? first.instance : -1;
+                    ids[1] = hit ? first.triangle : -1;
+                }
+                if (!R.rgbd) continue;
+                rgb = (unsigned char *)out_tbl.columns[R.rgbCol] + off;
             }
-            if (R.hitIDs) {
-                i32 *ids = R.hitIDs + ((size_t)view.outputRow * pixels_per_view + pix) * 2;
-                ids[0] = hit ? first.instance : -1;
-                ids[1] = hit ? first.triangle : -1;
-            }
-            if (!R.rgbd) continue;
-
-            unsigned char *rgb = (unsigned char *)out_tbl.columns[R.rgbCol] + off;
             Vector3 color { 0.f, 0.f, 0.f };
             if (hit) {
                 // colour of the hit (bvh_raycast.cpp:756-815)
@@ -1705,6 +1730,17 @@ static std::vector<LightCarrierArchetype> &lightCarriers(Executor *ex)
     return all.back().second;
 }
 
+// every output of a view is 4 bytes per pixel, and a view's output is one component
+static bool imageFitsComponent(u32 width, u32 height, std::string *err)
+{
+    if ((uint64_t)width * height * 4 > 0xffffffffull) {
+        *err = "render image of " + std::to_string(width) + " x " + std::to_string(height) +
+               " pixels: its 4-byte-per-pixel output buffers exceed the 32-bit component size";
+        return false;
+    }
+    return true;
+}
+
 // The image is render_width x render_height when both are set, else the render_resolution
 // square; segmentation, projection and normals are 0 or 1.
 bool renderParseConfig(const mb2_render_config *rc, RenderSettings *out, std::string *err)
@@ -1723,11 +1759,7 @@ bool renderParseConfig(const mb2_render_config *rc, RenderSettings *out, std::st
     }
     out->width = w != 0 ? w : res;
     out->height = h != 0 ? h : res;
-    if ((uint64_t)out->width * out->height * 4 > 0xffffffffull) {
-        *err = "render image of " + std::to_string(out->width) + " x " + std::to_string(out->height) +
-               " pixels: its 4-byte-per-pixel output buffers exceed the 32-bit component size";
-        return false;
-    }
+    if (!imageFitsComponent(out->width, out->height, err)) return false;
     if (rc->segmentation > 1) {
         *err = "segmentation = " + std::to_string(rc->segmentation) + " is not 0 (off) or 1 (on)";
         return false;
@@ -1938,6 +1970,7 @@ void renderHostDestroy(Executor *ex)
 {
     RenderHost *rh = ex->render;
     if (rh) {
+        if (rh->freeViews) cudaFree(rh->freeViews);
         vmRelease(&rh->instanceRange);
         vmRelease(&rh->nodeRange);
         vmRelease(&rh->keyRange);
@@ -2009,16 +2042,39 @@ void *renderDebugBuffer(Executor *ex, int which)
     }
 }
 
-// the flat-list and the TLAS instantiation of the ray caster, on the executor's stream
-template <bool MATERIALS, bool PANORAMA>
-static void launchRaycastPair(Executor *ex, unsigned view_blocks, u32 normals)
+// the flat-list and the TLAS instantiation of the ray caster
+template <bool MATERIALS, bool PANORAMA, bool FREE>
+static void launchRaycastPair(Executor *ex, dim3 grid, bool normals, const RaycastViews &job, cudaStream_t s)
 {
     if (normals) {
-        renderRaycastKernel<true, MATERIALS, PANORAMA, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
-        renderRaycastKernel<false, MATERIALS, PANORAMA, true><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+        renderRaycastKernel<true, MATERIALS, PANORAMA, true, FREE><<<grid, 256, 0, s>>>(ex->dState, job);
+        renderRaycastKernel<false, MATERIALS, PANORAMA, true, FREE><<<grid, 256, 0, s>>>(ex->dState, job);
     } else {
-        renderRaycastKernel<true, MATERIALS, PANORAMA, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
-        renderRaycastKernel<false, MATERIALS, PANORAMA, false><<<dim3(1, view_blocks), 256, 0, ex->stream>>>(ex->dState);
+        renderRaycastKernel<true, MATERIALS, PANORAMA, false, FREE><<<grid, 256, 0, s>>>(ex->dState, job);
+        renderRaycastKernel<false, MATERIALS, PANORAMA, false, FREE><<<grid, 256, 0, s>>>(ex->dState, job);
+    }
+}
+
+template <bool MATERIALS, bool PANORAMA>
+static void launchRaycastPair(Executor *ex, dim3 grid, bool normals, const RaycastViews &job, cudaStream_t s)
+{
+    if (job.views) launchRaycastPair<MATERIALS, PANORAMA, true>(ex, grid, normals, job, s);
+    else launchRaycastPair<MATERIALS, PANORAMA, false>(ex, grid, normals, job, s);
+}
+
+// every combination a launch can ask for maps onto these instantiations: the projection and the
+// normal output come from the caller, MATERIALS from the executor's config, FREE from the job
+static void launchRaycast(Executor *ex, dim3 grid, bool panorama, bool normals, const RaycastViews &job,
+                          cudaStream_t s)
+{
+    const bool materials = ex->render->hRender.materials != nullptr;
+    if (panorama) {
+        if (materials) launchRaycastPair<true, true>(ex, grid, normals, job, s);
+        else launchRaycastPair<false, true>(ex, grid, normals, job, s);
+    } else if (materials) {
+        launchRaycastPair<true, false>(ex, grid, normals, job, s);
+    } else {
+        launchRaycastPair<false, false>(ex, grid, normals, job, s);
     }
 }
 
@@ -2044,14 +2100,7 @@ LaunchGraph *physicsBuildRenderGraph(Executor *ex, std::string *err)
     // the live view count: one block per capacity row cost 76 us of empty-block scheduling at
     // 1024 worlds); 8 rounds of resident blocks keep the tail short
     const unsigned view_blocks = (unsigned)std::max(1, std::min(R.maxViews, ex->numSMs * kRaycastMinBlocks * 8));
-    if (R.projection == 1) {
-        if (R.materials) launchRaycastPair<true, true>(ex, view_blocks, R.normals);
-        else launchRaycastPair<false, true>(ex, view_blocks, R.normals);
-    } else if (R.materials) {
-        launchRaycastPair<true, false>(ex, view_blocks, R.normals);
-    } else {
-        launchRaycastPair<false, false>(ex, view_blocks, R.normals);
-    }
+    launchRaycast(ex, dim3(1, view_blocks), R.projection == 1, R.normals != 0, RaycastViews {}, ex->stream);
     launchStatusCopy(ex, ex->stream);
     cudaError_t e = cudaStreamEndCapture(ex->stream, &g->graph);
     if (e != cudaSuccess || cudaGraphInstantiate(&g->exec, g->graph, 0) != cudaSuccess) {
@@ -2062,6 +2111,103 @@ LaunchGraph *physicsBuildRenderGraph(Executor *ex, std::string *err)
     }
     g->numKernels = 3;
     return g;
+}
+
+bool renderFreeViews(Executor *ex, const mb2_free_view *views, uint32_t n, uint32_t width, uint32_t height,
+                     uint32_t projection, const mb2_free_view_outputs &out, cudaStream_t s, std::string *err)
+{
+    RenderHost *rh = ex->render;
+    if (!rh || !rh->active) {
+        *err = "the executor has no renderer (no CudaBatchRenderConfig was given, or the simulator never called "
+               "RenderingSystem::registerTypes)";
+        return false;
+    }
+    if (n == 0) {
+        *err = "num_views is 0";
+        return false;
+    }
+    if (width == 0 || height == 0) {
+        *err = "image of " + std::to_string(width) + " x " + std::to_string(height) +
+               " pixels: width and height must be at least 1";
+        return false;
+    }
+    if (!imageFitsComponent(width, height, err)) return false;
+    if (projection > 1) {
+        *err = "projection = " + std::to_string(projection) + " is not 0 (pinhole) or 1 (panorama)";
+        return false;
+    }
+    if (!out.rgb && !out.depth && !out.segmentation && !out.normals) {
+        *err = "every output (rgb, depth, segmentation, normals) is NULL";
+        return false;
+    }
+    const u32 num_worlds = ex->hState->numWorlds;
+    for (u32 i = 0; i < n; i++) {
+        const mb2_free_view &v = views[i];
+        const std::string at = "view " + std::to_string(i) + ": ";
+        if (v.world < 0 || (u32)v.world >= num_worlds) {
+            *err = at + "world " + std::to_string(v.world) + " is outside [0, " + std::to_string(num_worlds) + ")";
+            return false;
+        }
+        bool finite = std::isfinite(v.vfov_degrees);
+        for (float x : v.position) finite = finite && std::isfinite(x);
+        for (float x : v.rotation) finite = finite && std::isfinite(x);
+        if (!finite) {
+            *err = at + "position, rotation or vfov_degrees is not finite";
+            return false;
+        }
+        if (!(v.vfov_degrees > 0.f && v.vfov_degrees < 180.f)) {
+            *err = at + "vfov_degrees = " + std::to_string(v.vfov_degrees) + " is outside (0, 180)";
+            return false;
+        }
+    }
+
+    // the staging buffer: RenderView records, then the caller's records.  It only grows; the old
+    // one is freed with cudaFree, which waits for the device, so no earlier call still reads it
+    cudaSetDevice(ex->gpu);
+    if (n > rh->freeViewCapacity) {
+        const u32 cap = std::max(n, std::min(2 * rh->freeViewCapacity, 0x7fffffffu));
+        if (rh->freeViews) cudaFree(rh->freeViews);
+        rh->freeViews = nullptr;
+        rh->freeViewCapacity = 0;
+        if (cudaMalloc((void **)&rh->freeViews, (size_t)cap * (sizeof(RenderView) + sizeof(mb2_free_view))) !=
+                cudaSuccess) {
+            rh->freeViews = nullptr;
+            *err = "free view staging buffer allocation failed";
+            return false;
+        }
+        rh->freeViewCapacity = cap;
+    }
+    RenderView *rviews = (RenderView *)rh->freeViews;
+    mb2_free_view *records = (mb2_free_view *)(rh->freeViews + (size_t)rh->freeViewCapacity * sizeof(RenderView));
+    // from pageable memory: the call returns once the views are staged, so the caller may reuse them
+    cudaMemcpyAsync(records, views, (size_t)n * sizeof(mb2_free_view), cudaMemcpyHostToDevice, s);
+    renderConvertFreeViews(records, rviews, n, s);
+
+    // blocks: enough tile chunks per view that the views fill the render graph's 8 rounds of
+    // resident blocks, each chunk at least one tile per warp
+    const u32 tile_w = height < 4 ? 32u : 8u, tile_h = 32u / tile_w;
+    const uint64_t tiles = (uint64_t)((width + tile_w - 1) / tile_w) * ((height + tile_h - 1) / tile_h);
+    const uint64_t warps = 256 / 32;
+    const uint64_t resident = (uint64_t)ex->numSMs * kRaycastMinBlocks * 8;
+    const uint64_t chunks = std::max<uint64_t>(1, std::min((resident + n - 1) / n, (tiles + warps - 1) / warps));
+    const uint64_t view_blocks = std::max<uint64_t>(1, std::min<uint64_t>(n, resident / chunks));
+    RaycastViews job;
+    job.views = rviews;
+    job.numViews = n;
+    job.width = width;
+    job.height = height;
+    job.rgb = (unsigned char *)out.rgb;
+    job.depth = (float *)out.depth;
+    job.segmentation = (i32 *)out.segmentation;
+    job.normals = (u32 *)out.normals;
+    launchRaycast(ex, dim3((unsigned)chunks, (unsigned)view_blocks), projection == 1, out.normals != nullptr, job, s);
+    launchStatusCopy(ex, s);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) {
+        *err = std::string("launch failed: ") + cudaGetErrorString(e);
+        return false;
+    }
+    return true;
 }
 
 // algorithmic bytes of one frame (SURVEY.md 8d): W x H x 4 B depth (+ 4 B RGBA8)

@@ -29,6 +29,14 @@ void *renderDebugBuffer(Executor *ex, int which);
 uint64_t renderBytesPerFrame(Executor *ex, int64_t num_views);
 // host copy of the ray caster's state (device pointers, capacities), null when it is not active
 const RenderState *renderHostState(Executor *ex);
+// mb2_render_free_views after its null checks: checks the rest before any CUDA call, then
+// enqueues the views' copy, their conversion, the ray caster and the status copy on s
+bool renderFreeViews(Executor *ex, const mb2_free_view *views, uint32_t num_views, uint32_t width,
+                     uint32_t height, uint32_t projection, const mb2_free_view_outputs &outputs, cudaStream_t s,
+                     std::string *err);
+// device records -> RenderView (render_free_views.cu, compiled without FMA contraction)
+struct RenderView;
+void renderConvertFreeViews(const mb2_free_view *in, RenderView *out, uint32_t n, cudaStream_t s);
 // algorithmic bytes of one launch of a physics node + a short name (profiling)
 uint64_t physicsNodeBytes(Executor *ex, const NodeRecord &rec, const char **name, int64_t *rows);
 

@@ -50,6 +50,20 @@ struct RenderView {
     i32 outputRow;        // row of the view's RaycastOutputArchetype entity
 };
 
+// Where a free-view launch (mb2_render_free_views, renderRaycastKernel<..., FREE = true>) takes
+// its views and writes their pixels: view i writes slice i of every output that is not null.
+// The render graph's launches pass an empty one and read their views, their count, the image
+// size and the output columns from RenderState and the output table at run time.
+struct RaycastViews {
+    const RenderView *views;
+    u32 numViews;
+    u32 width, height;
+    unsigned char *rgb;     // [numViews][height][width][4]
+    float *depth;           // [numViews][height][width]
+    i32 *segmentation;      // [numViews][height][width]
+    u32 *normals;           // [numViews][height][width] of int8 x, y, z, w
+};
+
 enum RenderCol : int { RCPosition = 0, RCRotation, RCScale, RCObjectID, RCRenderable, RCCount };
 
 // == the LightDesc component as the simulator's compiler lays it out

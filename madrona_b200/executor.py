@@ -56,6 +56,7 @@ EXPORTED_SYMBOLS = [
     "mb2_navmesh_destroy",
     "mb2_render_debug_hits",
     "mb2_render_debug_buffer",
+    "mb2_render_free_views",
     "mb2_peer_gather_create",
     "mb2_peer_gather_local_handle",
     "mb2_peer_gather_connect",
@@ -136,6 +137,20 @@ class _RenderConfigC(ctypes.Structure):      # == madrona::CudaBatchRenderConfig
         # normal x 127 in the view's frame (w = 0), all zero on a miss
         ("normals", ctypes.c_uint32),
     ]
+
+
+class _FreeViewC(ctypes.Structure):         # == mb2_free_view
+    _fields_ = [
+        ("world", ctypes.c_int32),
+        ("position", ctypes.c_float * 3),   # the camera's world position (entity + camera offset)
+        ("rotation", ctypes.c_float * 4),   # the viewing entity's Rotation, w, x, y, z
+        ("vfov_degrees", ctypes.c_float),
+    ]
+
+
+class _FreeViewOutputsC(ctypes.Structure):  # == mb2_free_view_outputs: device pointers or NULL
+    _fields_ = [("rgb", ctypes.c_void_p), ("depth", ctypes.c_void_p),
+                ("segmentation", ctypes.c_void_p), ("normals", ctypes.c_void_p)]
 
 
 class _SourceHullC(ctypes.Structure):
@@ -284,6 +299,9 @@ def load_library() -> ctypes.CDLL:
     lib.mb2_render_debug_hits.restype = vp
     lib.mb2_render_debug_buffer.argtypes = [vp, ctypes.c_int, ctypes.POINTER(ctypes.c_int64)]
     lib.mb2_render_debug_buffer.restype = vp
+    lib.mb2_render_free_views.argtypes = [vp, ctypes.POINTER(_FreeViewC), ctypes.c_uint32, ctypes.c_uint32,
+                                          ctypes.c_uint32, ctypes.c_uint32, ctypes.POINTER(_FreeViewOutputsC), vp]
+    lib.mb2_render_free_views.restype = ctypes.c_int
     lib.mb2_peer_gather_create.argtypes = [vp, ctypes.POINTER(ctypes.c_int64), ctypes.c_uint32,
                                            ctypes.POINTER(ctypes.c_uint64), ctypes.c_uint32, ctypes.c_uint32]
     lib.mb2_peer_gather_create.restype = vp
@@ -543,6 +561,56 @@ class MWCudaExecutor:
         nodes = fetch(1, (max(total, 1), 60), "|u1")[:total]
         inst = fetch(3, (max(total, 1), 80), "|u1")[:total, :76]
         return nodes, ncount, inst, icount, offsets
+
+    def renderFreeViews(self, views, width: int, height: int, panorama: bool = False, rgb: bool = True,
+                        depth: bool = True, segmentation: bool = False, normals: bool = False, stream=None):
+        """Ray-cast caller-given views of the scene the last render-prepare built
+        (mb2_render_free_views in include/madrona_b200.h).  `views` is a sequence of
+        (world, position xyz, rotation wxyz, vfov_degrees) or a numpy structured array with those
+        fields; a view with the pose and field of view of one of the simulator's cameras, at the
+        executor's size and projection, gives that camera's bytes.  Returns a dict of torch
+        tensors on this executor's GPU, view i at index i: "rgb" uint8 [n, H, W, 4], "depth"
+        float32 [n, H, W], "segmentation" int32 [n, H, W], "normals" int8 [n, H, W, 4], those
+        asked for.  stream=None: synchronous on the executor's stream, like run(); a
+        torch.cuda.Stream or raw handle: enqueued there, the tensors recorded on it."""
+        import numpy as np
+        import torch
+        dt = np.dtype(_FreeViewC)
+        if isinstance(views, np.ndarray) and views.dtype.names:
+            arr = np.empty(len(views), dtype=dt)
+            for name in dt.names:
+                arr[name] = views[name]
+        else:
+            rows = list(views)
+            arr = np.empty(len(rows), dtype=dt)
+            arr["world"] = [int(r[0]) for r in rows]
+            arr["position"] = np.asarray([np.asarray(r[1], dtype=np.float32) for r in rows],
+                                         dtype=np.float32).reshape(len(rows), 3)
+            arr["rotation"] = np.asarray([np.asarray(r[2], dtype=np.float32) for r in rows],
+                                         dtype=np.float32).reshape(len(rows), 4)
+            arr["vfov_degrees"] = [float(r[3]) for r in rows]
+        n = len(arr)
+        dev = torch.device("cuda", self.gpu_id)
+        shapes = {"rgb": ((n, height, width, 4), torch.uint8), "depth": ((n, height, width), torch.float32),
+                  "segmentation": ((n, height, width), torch.int32), "normals": ((n, height, width, 4), torch.int8)}
+        wanted = {"rgb": rgb, "depth": depth, "segmentation": segmentation, "normals": normals}
+        with torch.cuda.device(dev):
+            out = {k: torch.empty(shapes[k][0], dtype=shapes[k][1], device=dev) for k in shapes if wanted[k]}
+            s = self.stream if stream is None else int(getattr(stream, "cuda_stream", stream))
+            target = torch.cuda.ExternalStream(s, device=dev)
+            # the new tensors are ordered on the current stream: the render waits for it
+            target.wait_stream(torch.cuda.current_stream(dev))
+            ptrs = _FreeViewOutputsC(*[out[k].data_ptr() if k in out else None for k in shapes])
+            if self._lib.mb2_render_free_views(self._h, arr.ctypes.data_as(ctypes.POINTER(_FreeViewC)), n,
+                                               int(width), int(height), 1 if panorama else 0, ctypes.byref(ptrs),
+                                               ctypes.c_void_p(s)) != 0:
+                raise MadronaB200Error(_last_error(self._lib))
+            if stream is None:
+                target.synchronize()
+            else:
+                for t in out.values():
+                    t.record_stream(target)
+        return out
 
     def peerGather(self, slots, shapes, dtypes, world_size: int, rank: int):
         """NVLink peer-store gather of fixed-size exported columns across the ranks of a

@@ -9,6 +9,7 @@
 // (reference FATAL(), include/madrona/crash.hpp).
 #pragma once
 
+#include <cstddef>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -174,6 +175,27 @@ struct RenderOutputs {
 enum class RenderProjection : uint32_t {
     Pinhole = 0,
     Panorama = 1,
+};
+
+// A view for MWCudaExecutor::renderFreeViews (== mb2_free_view): the world, the camera's world
+// position (entity position plus camera offset), the viewing entity's Rotation (w, x, y, z; the
+// camera looks along the rotated +y axis) and the vertical field of view, as attachEntityToView
+// takes it.
+struct FreeView {
+    int32_t world;
+    float position[3];
+    float rotation[4];
+    float vfovDegrees;
+};
+
+// Device pointers, or nullptr for an output not wanted, in the exported columns' layouts with
+// view i at slice i: rgb uint8 [n][H][W][4], depth float [n][H][W], segmentation int32 [n][H][W],
+// normals int8 [n][H][W][4].
+struct FreeViewOutputs {
+    void *rgb;
+    void *depth;
+    void *segmentation;
+    void *normals;
 };
 
 // A device-memory snapshot of an executor's simulation state (include/madrona_b200.h),
@@ -356,6 +378,25 @@ public:
     }
 
     void *getExported(CountT slot) const { return mb2_get_exported(h_, (int64_t)slot); }
+
+    // Not in the reference: ray-cast `views` of the scene the last step prepared into the
+    // caller's buffers, every view image_size pixels with `projection`, enqueued on `strm`
+    // (nullptr: the executor's stream) like runAsync (include/madrona_b200.h,
+    // mb2_render_free_views).  A view with a camera's pose, field of view, size and projection
+    // writes the render graph's bytes for that camera.
+    void renderFreeViews(Span<const ::madrona_b200::FreeView> views, ::madrona_b200::RenderImageSize image_size,
+                         ::madrona_b200::RenderProjection projection, ::madrona_b200::FreeViewOutputs outputs,
+                         cudaStream_t strm = nullptr)
+    {
+        static_assert(sizeof(::madrona_b200::FreeView) == sizeof(mb2_free_view) &&
+                      offsetof(::madrona_b200::FreeView, vfovDegrees) == offsetof(mb2_free_view, vfov_degrees),
+                      "FreeView layout");
+        const mb2_free_view_outputs out { outputs.rgb, outputs.depth, outputs.segmentation, outputs.normals };
+        if (mb2_render_free_views(h_, (const mb2_free_view *)views.data(), (uint32_t)views.size(), image_size.width,
+                                  image_size.height, (uint32_t)projection, &out, (void *)strm) != 0) {
+            detail::fatal("renderFreeViews");
+        }
+    }
 
     // Not in the reference: a snapshot of this executor's state (empty until its first save)
     ::madrona_b200::ExecutorSnapshot snapshot()
