@@ -40,12 +40,20 @@ void Sim::registerTypes(ECSRegistry &registry, const Config &)
     registry.exportColumn<Body, Velocity>((uint32_t)ExportID::BodyVel);
     registry.exportColumn<Body, Entity>((uint32_t)ExportID::BodyEntity);
     registry.exportSingleton<BodyCount>((uint32_t)ExportID::BodyCount);
+#ifdef CROWD_TWO_ARCHETYPES
+    registry.registerArchetype<Body2>();
+    registry.exportColumn<Body2, Position>((uint32_t)ExportID::Body2Pos);
+    registry.exportColumn<Body2, Rotation>((uint32_t)ExportID::Body2Rot);
+    registry.exportColumn<Body2, Velocity>((uint32_t)ExportID::Body2Vel);
+    registry.exportColumn<Body2, Entity>((uint32_t)ExportID::Body2Entity);
+#endif
 }
 
+template <typename ArchetypeT = Body>
 static inline Entity makeBody(Engine &ctx, Vector3 pos, Quat rot, Diag3x3 scale,
                               SimObject obj, ResponseType resp, Vector3 lin_vel)
 {
-    Entity e = ctx.makeEntity<Body>();
+    Entity e = ctx.makeEntity<ArchetypeT>();
     ObjectID obj_id { (int32_t)obj };
     ctx.get<Position>(e) = pos;
     ctx.get<Rotation>(e) = rot;
@@ -144,10 +152,19 @@ static void spawnWorld(Engine &ctx)
             vel.y = 6.f * (rng.sampleUniform() - 0.5f);
         }
         const Quat rot = obj == SimObject::Ball ? upright : randomQuat(rng);
+#ifdef CROWD_TWO_ARCHETYPES
+        if (i % kSecondEvery == kSecondEvery - 1) {
+            sim.bodies[n++] = makeBody<Body2>(ctx, pos, rot, scale, obj, ResponseType::Dynamic, vel);
+            continue;
+        }
+#endif
         sim.bodies[n++] = makeBody(ctx, pos, rot, scale, obj, ResponseType::Dynamic, vel);
     }
     sim.numBodies = n;
     ctx.singleton<BodyCount>().count = n;
+#ifdef CROWD_TWO_ARCHETYPES
+    ctx.singleton<BodyCount>().second = num_dyn / kSecondEvery;
+#endif
 }
 
 // One invocation per world: at the end of an episode, destroy every body and respawn

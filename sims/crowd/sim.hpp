@@ -13,6 +13,11 @@
 // bodies towards one corner in a geometric spiral, a tree deeper than the rebuild's
 // 64-entry stacks: the engine must refuse it (GPU only).
 //
+// Built with -DCROWD_TWO_ARCHETYPES=1 (the crowd2 fixture), every kSecondEvery-th dynamic
+// body is a Body2 instead of a Body: a second rigid-body archetype, whose slots in a world's
+// body list follow all of Body's.  Its columns are exported after BodyCount, and BodyCount
+// also holds how many of the world's bodies are Body2s.
+//
 // Compiled unchanged for the reference CPU backend (oracle/harness_crowd.cpp) and,
 // through NVRTC, for this engine.
 #pragma once
@@ -40,6 +45,9 @@ constexpr int32_t kNumStatic = 5;          // plane and four walls
 constexpr int32_t kMaxBodies = 4096;       // per world, static bodies included
 constexpr int32_t kVariedMaxBodies = 1500; // the largest of kEpisodeSizes
 constexpr int32_t kNumEpisodeSizes = 7;
+#ifdef CROWD_TWO_ARCHETYPES
+constexpr int32_t kSecondEvery = 4;        // dynamic body i is a Body2 when i % 4 == 3
+#endif
 
 enum class ExportID : uint32_t {
     BodyPos,
@@ -47,6 +55,12 @@ enum class ExportID : uint32_t {
     BodyVel,
     BodyEntity,
     BodyCount,
+#ifdef CROWD_TWO_ARCHETYPES
+    Body2Pos,
+    Body2Rot,
+    Body2Vel,
+    Body2Entity,
+#endif
     NumExports,
 };
 
@@ -80,9 +94,15 @@ enum class Layout : uint32_t {
 
 struct BodyCount {
     int32_t count;
+#ifdef CROWD_TWO_ARCHETYPES
+    int32_t second;            // of which Body2s
+#endif
 };
 
 struct Body : public madrona::Archetype<madrona::phys::RigidBody> {};
+#ifdef CROWD_TWO_ARCHETYPES
+struct Body2 : public madrona::Archetype<madrona::phys::RigidBody> {};
+#endif
 
 struct Config {
     madrona::phys::ObjectManager *objMgr;

@@ -136,6 +136,34 @@ def _hullpile_desc(name, bodies, compile_flags=(), objects=_hullpile_objects):
     )
 
 
+def _crowd_desc(name, two_archetypes=False):
+    outputs = [Slot(0, "body_pos", "float32", (3,), dynamic=True),
+               Slot(1, "body_rot", "float32", (4,), dynamic=True),
+               Slot(2, "body_vel", "float32", (6,), dynamic=True),
+               Slot(3, "body_entity", "int32", (2,), dynamic=True),
+               Slot(4, "body_count", "int32", (2 if two_archetypes else 1,))]
+    if two_archetypes:
+        outputs += [Slot(5, "body2_pos", "float32", (3,), dynamic=True),
+                    Slot(6, "body2_rot", "float32", (4,), dynamic=True),
+                    Slot(7, "body2_vel", "float32", (6,), dynamic=True),
+                    Slot(8, "body2_entity", "int32", (2,), dynamic=True)]
+    return SimDesc(
+        name=name,
+        sources=[os.path.join(_ROOT, "crowd", "sim.cpp")],
+        num_exports=len(outputs),
+        num_taskgraphs=1,
+        inputs=[],
+        outputs=outputs,
+        pack_config=lambda cfg: struct.pack("<QIIII", int(cfg.get("obj_mgr_ptr", 0)), int(cfg["episode_len"]),
+                                            int(cfg["uniform_bodies"]), int(cfg["layout"]), 0),
+        pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
+        oracle_extra=lambda cfg: [int(cfg.get("seed", 0)), int(cfg["episode_len"]), int(cfg["uniform_bodies"])],
+        defaults={"seed": 0, "episode_len": 40, "uniform_bodies": 0, "layout": 0},
+        objects=_hullpile_objects,
+        compile_flags=["-DCROWD_TWO_ARCHETYPES=1"] if two_archetypes else [],
+    )
+
+
 def _image_size(cfg, default_res):
     """Render config image size from the fixture config: keyword arguments for the
     render_assets builders.  `width` and `height` (both) give non-square images, else the
@@ -460,24 +488,10 @@ SIMS: Dict[str, SimDesc] = {
     # worlds of 20 to 1500 bodies whose sizes change every episode (or uniform_bodies for all),
     # past the 128-body warp-per-world candidate search (tests/test_large_physics_worlds.py);
     # layout 1 clusters the bodies into a tree deeper than the rebuild's stacks (GPU only)
-    "crowd": SimDesc(
-        name="crowd",
-        sources=[os.path.join(_ROOT, "crowd", "sim.cpp")],
-        num_exports=5,
-        num_taskgraphs=1,
-        inputs=[],
-        outputs=[Slot(0, "body_pos", "float32", (3,), dynamic=True),
-                 Slot(1, "body_rot", "float32", (4,), dynamic=True),
-                 Slot(2, "body_vel", "float32", (6,), dynamic=True),
-                 Slot(3, "body_entity", "int32", (2,), dynamic=True),
-                 Slot(4, "body_count", "int32", (1,))],
-        pack_config=lambda cfg: struct.pack("<QIIII", int(cfg.get("obj_mgr_ptr", 0)), int(cfg["episode_len"]),
-                                            int(cfg["uniform_bodies"]), int(cfg["layout"]), 0),
-        pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
-        oracle_extra=lambda cfg: [int(cfg.get("seed", 0)), int(cfg["episode_len"]), int(cfg["uniform_bodies"])],
-        defaults={"seed": 0, "episode_len": 40, "uniform_bodies": 0, "layout": 0},
-        objects=_hullpile_objects,
-    ),
+    "crowd": _crowd_desc("crowd"),
+    # build variant with a second rigid-body archetype (every 4th dynamic body): its columns
+    # as slots 5 - 8, and body_count also holds how many of the world's bodies it has
+    "crowd2": _crowd_desc("crowd2", two_archetypes=True),
     "gridworld": SimDesc(
         name="gridworld",
         sources=[os.path.join(_ROOT, "gridworld", "sim.cpp")],
