@@ -305,6 +305,48 @@ int mb2_render_free_views(mb2_executor *exec, const mb2_free_view *views, uint32
                           uint32_t width, uint32_t height, uint32_t projection,
                           const mb2_free_view_outputs *outputs, void *cuda_stream);
 
+/* ---- physics ray queries ------------------------------------------------------
+ * No reference counterpart.  Traces a batch of rays against the worlds' collision
+ * geometry (the broadphase trees the last step left): ray i gives what
+ *     ctx.singleton<broadphase::BVH>().traceRay(origin[i], direction[i], &t, &normal, max_t[i])
+ * returns in world world[i] when called by a system placed as the last node of the launch
+ * graph that ran last -- bit for bit with the simulator compiled without FMA contraction
+ * (MADRONA_B200_FAST_MATH=0, the default), and for hulls and planes the reference CPU
+ * backend's BVH::traceRay.
+ *   - rays: SoA, contiguous: world int32 [n], origin float [n][3], direction float [n][3]
+ *     (not normalised; t is in units of its length), max_t float [n] or NULL for +inf.  Rays
+ *     may come in any world order, with repeats.
+ *   - hits: entity int32 [n][2] {gen, id}, t float [n], normal float [n][3] (world frame); an
+ *     output left NULL is not written.  A miss writes entity {0xFFFFFFFF, -1}
+ *     (Entity::none()), t = 0 and normal (0, 0, 0): the entity is the hit flag, since a ray
+ *     that starts on a face can hit at t = 0.  A ray that starts inside a hull does not report
+ *     that hull; sphere primitives are never hit (traceRay skips them).  Before the first
+ *     step every ray misses; after a snapshot restore rays see the saved trees.
+ *   - Every pointer is a device pointer, 4-byte aligned.  Nothing but the outputs is written.
+ *   - Enqueued on cuda_stream (NULL: the executor's stream), never synchronizing the host.  It
+ *     reads the trees the step graph rewrites, so it is part of the "one launch graph in
+ *     flight" rule: put it on the stream of the steps or chain the streams with events, and
+ *     do not overlap two calls on one executor (they share its scratch).
+ *   - A world[i] outside [0, num_worlds) writes a miss for that ray and fails the next mb2_run
+ *     (a device-side error, like a physics buffer overflow).
+ *   - Returns 0 (n == 0 is a no-op), or 1 with a message in mb2_last_error() and nothing
+ *     launched for: a null executor or rays, an executor whose simulator never registered
+ *     PhysicsSystem, a NULL world, origin or direction, all three outputs NULL, or a pointer
+ *     that is not 4-byte aligned. */
+typedef struct mb2_physics_rays {
+    const int32_t *world;
+    const float *origin;
+    const float *direction;
+    const float *max_t;
+} mb2_physics_rays;
+typedef struct mb2_physics_ray_hits {
+    int32_t *entity;               /* [n][2] {gen, id} */
+    float *t;
+    float *normal;                 /* [n][3] */
+} mb2_physics_ray_hits;
+int mb2_trace_physics_rays(mb2_executor *exec, const mb2_physics_rays *rays, uint32_t n,
+                           const mb2_physics_ray_hits *hits, void *cuda_stream);
+
 /* Kernel nodes inside a built launch graph (== launches per run). */
 int64_t mb2_launch_graph_num_kernels(const mb2_launch_graph *graph);
 

@@ -78,6 +78,8 @@ static std::string describeErrors(uint32_t flags, uint32_t archetype)
     if (flags & ErrPhysicsOverflow) s += "physics buffer overflow ";
     if (flags & ErrRenderAsset) s += "render asset error (a material's textureIdx is not below "
         "materialData.numTextureBuffers; those pixels were shaded untextured) ";
+    if (flags & ErrPhysicsRayWorld) s += "physics ray query with a world outside [0, num_worlds) "
+        "(mb2_trace_physics_rays wrote a miss for that ray) ";
     if (flags & ErrRenderCapacity) s += "render instance list overflow ";
     if (flags & ErrRenderTLASDepth) s += "render TLAS too deep for the ray caster's traversal stack (a world's "
         "renderables are too tightly clustered) ";
@@ -645,6 +647,7 @@ static void destroyExecutor(Executor *ex)
     if (!ex) return;
     cudaSetDevice(ex->gpu);
     if (ex->stream) cudaStreamSynchronize(ex->stream);
+    physicsRaysDestroy(ex);
     physicsHostDestroy(ex);
     renderHostDestroy(ex);
     sortScratchDestroy(ex);
@@ -1362,6 +1365,24 @@ int mb2_render_free_views(mb2_executor *exec, const mb2_free_view *views, uint32
     if (!renderFreeViews(ex, views, num_views, width, height, projection, out,
                          cuda_stream ? (cudaStream_t)cuda_stream : ex->stream, &err)) {
         setError("mb2_render_free_views: " + err);
+        return 1;
+    }
+    return 0;
+}
+
+int mb2_trace_physics_rays(mb2_executor *exec, const mb2_physics_rays *rays, uint32_t n,
+                           const mb2_physics_ray_hits *hits, void *cuda_stream)
+{
+    g_last_error.clear();
+    if (!exec || !rays) {
+        setError("mb2_trace_physics_rays: null executor or rays");
+        return 1;
+    }
+    Executor *ex = (Executor *)exec;
+    const mb2_physics_ray_hits out = hits ? *hits : mb2_physics_ray_hits {};
+    std::string err;
+    if (!physicsTraceRays(ex, *rays, n, out, cuda_stream ? (cudaStream_t)cuda_stream : ex->stream, &err)) {
+        setError("mb2_trace_physics_rays: " + err);
         return 1;
     }
     return 0;

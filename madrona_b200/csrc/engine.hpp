@@ -15,6 +15,7 @@ namespace mb2 {
 struct SortScratch;   // kernels_sort.cu
 struct PhysicsHost;   // kernels_physics.cu
 struct RenderHost;    // kernels_render.cu
+struct PhysicsRayHost;   // physics_rays.cu
 
 // The MADRONA_B200_* environment variables that configure an executor, as parseKnobs read them
 struct Knobs {
@@ -68,6 +69,7 @@ struct Executor {
     SortScratch *sortScratch = nullptr;
     PhysicsHost *physics = nullptr;
     RenderHost *render = nullptr;
+    PhysicsRayHost *physicsRays = nullptr;   // scratch of mb2_trace_physics_rays, made by its first call
 
     Knobs knobs;                     // read and checked before any CUDA call
     RenderSettings renderSettings;   // likewise, from the render config

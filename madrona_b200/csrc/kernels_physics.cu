@@ -3214,6 +3214,12 @@ void physicsBeforeGraphCapture(Executor *ex)
     physicsClassifyPrims(ex);
 }
 
+const PhysicsState *physicsHostState(Executor *ex)
+{
+    const PhysicsHost *ph = ex->physics;
+    return ph && ph->active ? &ph->hPhys : nullptr;
+}
+
 void physicsHostDestroy(Executor *ex)
 {
     delete ex->physics;

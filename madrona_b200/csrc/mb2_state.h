@@ -240,6 +240,7 @@ enum ErrorFlags : u32 {
     ErrRenderTLASDepth = 1u << 9,      // a world's TLAS is too deep for the ray caster's stack
     ErrTooManyNodeDatas = 1u << 10,    // more custom node datas than kMaxNodeDatas
     ErrNavmeshPolygon = 1u << 11,      // Navmesh::initFromPolygons got a polygon of fewer than 3 vertices
+    ErrPhysicsRayWorld = 1u << 12,     // mb2_trace_physics_rays got a ray of a world outside [0, numWorlds)
 };
 
 }

@@ -31,8 +31,11 @@ struct HalfEdgeMesh {
     uint32_t numVertices;
 };
 
+// CollisionPrimitive::type (== phys::CollisionPrimitive::Type)
+constexpr uint32_t kPrimSphere = 1, kPrimHull = 2, kPrimPlane = 4;
+
 struct CollisionPrimitive {
-    uint32_t type;     // 1 sphere, 2 hull, 4 plane
+    uint32_t type;     // kPrimSphere, kPrimHull or kPrimPlane
     union {
         float sphereRadius;
         HalfEdgeMesh hull;

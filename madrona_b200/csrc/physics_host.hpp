@@ -6,6 +6,8 @@
 
 namespace mb2 {
 
+struct PhysicsState;
+
 bool physicsHostCreate(Executor *ex, std::string *err);
 bool physicsHostAfterRegistry(Executor *ex, std::string *err);
 void physicsHostDestroy(Executor *ex);
@@ -37,6 +39,14 @@ bool renderFreeViews(Executor *ex, const mb2_free_view *views, uint32_t num_view
 // device records -> RenderView (render_free_views.cu, compiled without FMA contraction)
 struct RenderView;
 void renderConvertFreeViews(const mb2_free_view *in, RenderView *out, uint32_t n, cudaStream_t s);
+// host copy of the physics state (device pointers, knobs), null when the simulator never called
+// PhysicsSystem::registerTypes
+const PhysicsState *physicsHostState(Executor *ex);
+// mb2_trace_physics_rays after its null checks: checks the rest before any CUDA call, then
+// enqueues the grouping of the rays by world and their traces on s (physics_rays.cu)
+bool physicsTraceRays(Executor *ex, const mb2_physics_rays &rays, uint32_t n, const mb2_physics_ray_hits &hits,
+                      cudaStream_t s, std::string *err);
+void physicsRaysDestroy(Executor *ex);
 // algorithmic bytes of one launch of a physics node + a short name (profiling)
 uint64_t physicsNodeBytes(Executor *ex, const NodeRecord &rec, const char **name, int64_t *rows);
 

@@ -89,10 +89,6 @@ private:
         return Entity { (uint32_t)(v & 0xFFFFFFFFull), (int32_t)(uint32_t)(v >> 32) };
     }
 
-    inline bool traceRayIntoLeaf(int32_t leaf_idx, math::Vector3 world_ray_o,
-                                 math::Vector3 world_ray_d, float t_min, float t_max,
-                                 float *hit_t, math::Vector3 *hit_normal);
-
     mb2::WorldBVH s_;
 };
 

@@ -21,6 +21,7 @@
 
 #include <madrona/broadphase.hpp>
 #include <madrona/geo.hpp>
+#include <physics_ray.h>
 
 namespace madrona::phys {
 
@@ -568,193 +569,19 @@ inline void findEntitiesWithinAABB(Context &ctx, math::AABB aabb, Fn &&fn)
 
 namespace broadphase {
 
-namespace detail {
-
-inline bool rayIntoPlane(math::Vector3 ray_o, math::Vector3 ray_d, float t_min,
-                         float t_max, float *hit_t, math::Vector3 *hit_normal)
-{
-    // object space: the plane is z = 0 with normal +z
-    float denom = ray_d.z;
-    if (denom == 0) return false;
-    float t = -ray_o.z / denom;
-    if (t < t_min || t > t_max) return false;
-    *hit_t = t;
-    *hit_normal = math::Vector3 { 0, 0, 1 };
-    return true;
-}
-
-// Ray vs convex polyhedron as an intersection of half-spaces (RTCD 5.3.8);
-// face normals point outwards.  A ray that only crosses back faces is a miss.
-inline bool rayIntoHull(const geo::HalfEdgeMesh &mesh, math::Vector3 ray_o,
-                        math::Vector3 ray_d, float t_min, float t_max,
-                        float *hit_t, math::Vector3 *hit_normal)
-{
-    float t_enter = t_min;
-    float t_exit = t_max;
-    math::Vector3 enter_normal = math::Vector3::zero();
-    const CountT num_faces = (CountT)mesh.numFaces;
-    for (CountT f = 0; f < num_faces; f++) {
-        geo::Plane plane = mesh.facePlanes[f];
-        float denom = dot(plane.normal, ray_d);
-        float neg_dist = plane.d - dot(plane.normal, ray_o);
-        if (denom == 0.0f) {
-            if (neg_dist < 0.0f) return false;
-        } else {
-            float t = neg_dist / denom;
-            if (denom < 0.0f) {
-                if (t >= t_enter) {
-                    t_enter = t;
-                    enter_normal = plane.normal;
-                }
-            } else if (t <= t_exit) {
-                t_exit = t;
-            }
-            if (t_enter > t_exit) return false;
-        }
-    }
-    if (enter_normal.x == 0 && enter_normal.y == 0 && enter_normal.z == 0) return false;
-    *hit_t = t_enter;
-    *hit_normal = enter_normal;
-    return true;
-}
-
-}
-
-bool BVH::traceRayIntoLeaf(int32_t leaf_idx, math::Vector3 world_ray_o,
-                           math::Vector3 world_ray_d, float t_min, float t_max,
-                           float *hit_t, math::Vector3 *hit_normal)
-{
-    const ObjectManager *obj_mgr = (const ObjectManager *)s_.objMgr;
-    const int32_t obj = s_.leafObjIDs[leaf_idx];
-    const mb2::LeafTransform txfm = s_.leafTransforms[leaf_idx];
-    const math::Quat rot { txfm.rot.w, txfm.rot.x, txfm.rot.y, txfm.rot.z };
-    const math::Vector3 pos { txfm.pos.x, txfm.pos.y, txfm.pos.z };
-    const math::Quat to_local = rot.inv();
-
-    math::Vector3 obj_o = to_local.rotateVec(world_ray_o - pos);
-    obj_o.x /= txfm.scale.x;
-    obj_o.y /= txfm.scale.y;
-    obj_o.z /= txfm.scale.z;
-    math::Vector3 obj_d = rot.inv().rotateVec(world_ray_d);
-    obj_d.x /= txfm.scale.x;
-    obj_d.y /= txfm.scale.y;
-    obj_d.z /= txfm.scale.z;
-    math::Diag3x3 inv_d = math::Diag3x3::fromVec(1.f / obj_d);
-
-    const CountT prim_offset = (CountT)obj_mgr->rigidBodyPrimitiveOffsets[obj];
-    const CountT num_prims = (CountT)obj_mgr->rigidBodyPrimitiveCounts[obj];
-
-    math::Vector3 obj_normal;
-    bool hit_leaf = false;
-    for (CountT i = 0; i < num_prims; i++) {
-        const CountT prim_idx = prim_offset + i;
-        math::AABB prim_aabb = obj_mgr->primitiveAABBs[prim_idx];
-        if (!prim_aabb.rayIntersects(obj_o, inv_d, 0.f, t_max)) continue;
-
-        const CollisionPrimitive *prim = &obj_mgr->collisionPrimitives[prim_idx];
-        bool hit = false;
-        if (prim->type == CollisionPrimitive::Type::Hull) {
-            hit = detail::rayIntoHull(prim->hull.halfEdgeMesh, obj_o, obj_d,
-                                      t_min, t_max, hit_t, &obj_normal);
-        } else if (prim->type == CollisionPrimitive::Type::Plane) {
-            hit = detail::rayIntoPlane(obj_o, obj_d, t_min, t_max, hit_t, &obj_normal);
-        }
-        if (hit) {
-            hit_leaf = true;
-            t_max = *hit_t;
-        }
-    }
-    if (!hit_leaf) return false;
-    *hit_normal = rot.rotateVec(obj_normal);
-    return true;
-}
-
+// The walk itself is csrc/physics_ray.h, which the engine's batched ray queries
+// (mb2_trace_physics_rays) compile too: both return the same bits for the same ray.
 Entity BVH::traceRay(math::Vector3 o, math::Vector3 d, float *out_hit_t,
                      math::Vector3 *out_hit_normal, float t_max)
 {
-    math::Diag3x3 inv_d = math::Diag3x3::fromVec(d).inv();
-
-    // The reference walks the 4-wide tree with a stack (src/physics/
-    // broadphase.cpp:658-724), testing child i of a popped node against the
-    // t_max current at that moment:
-    //   max(mins.x, mins.y, mins.z, 0) <= min(maxes.x, maxes.y, maxes.z, t_max)
-    // (math.inl:1670-1696, NaN-skipping fminf / fmaxf).  A leaf is entered iff
-    // its own slot box passes that test when its turn comes: every ancestor box
-    // contains it (the slab expressions are monotonic in the box bounds and
-    // t_max only shrinks), and leaves are met in the tree's fixed report order.
-    // So the walk is a linear scan over WorldBVH::orderedBoxes -- same leaves,
-    // same order, same floats, no stack and no node pointer chasing.
-    //
-    //
-    // Mechanism (results identical by construction): boxes are handled in chunks of 64.
-    //   1. uniform pass: every lane slab-tests the chunk's boxes against its CURRENT t_max and
-    //      keeps the passing ones as a 64-bit mask -- all lanes run the same loop, no divergence.
-    //      t_max only shrinks afterwards and a smaller t_max can only turn a pass into a fail
-    //      (exit = min(..., t_max)), so the mask is a superset of the leaves the walk enters;
-    //   2. ordered pass over the mask bits: the slab test is REPEATED with the t_max of that
-    //      moment -- the reference's exact decision, same expression, same floats -- and the
-    //      leaves that pass are entered in order.  Each round every lane first moves on to its
-    //      next entered leaf, then the lanes that called together run the (expensive) leaf
-    //      test together; the warp votes keep the compiler from folding the two phases back
-    //      into one divergent loop.
-    // (The one-phase scan over all boxes spent most of its instructions in the divergent
-    // "walk to my next entered leaf" loop with most lanes idle.  Seeding t_max with the hit
-    // of the nearest-entry leaf before the walk is an extra pass over the boxes.)
-    const unsigned peers = __activemask();
-    const mb2::PVec4 *boxes = s_.orderedBoxes;
-    const int32_t num_boxes = s_.numTraversal;
-    Entity closest = Entity::none();
-    math::Vector3 closest_normal { 0, 0, 0 };
-
-    auto entered = [&](int32_t j, int32_t *leaf) {
-        const mb2::PVec4 b0 = boxes[2 * j], b1 = boxes[2 * j + 1];
-        const float lx = inv_d.d0 * (b0.x - o.x), ux = inv_d.d0 * (b0.w - o.x);
-        const float ly = inv_d.d1 * (b0.y - o.y), uy = inv_d.d1 * (b1.x - o.y);
-        const float lz = inv_d.d2 * (b0.z - o.z), uz = inv_d.d2 * (b1.y - o.z);
-        const float entry = fmaxf(fminf(lx, ux), fmaxf(fminf(ly, uy), fmaxf(fminf(lz, uz), 0.f)));
-        const float exit = fminf(fmaxf(lx, ux), fminf(fmaxf(ly, uy), fminf(fmaxf(lz, uz), t_max)));
-        *leaf = __float_as_int(b1.z);
-        return entry <= exit;
-    };
-
-    // (every peer runs the same number of chunk iterations: lanes of one warp may belong to
-    // worlds with different leaf counts)
-    for (int32_t base = 0; __any_sync(peers, base < num_boxes); base += 64) {
-        const int32_t left = num_boxes - base;
-        const int32_t chunk = left < 0 ? 0 : (left < 64 ? left : 64);
-        unsigned long long cand = 0;
-        for (int32_t j = 0; j < chunk; j++) {
-            int32_t leaf;
-            if (entered(base + j, &leaf)) cand |= 1ull << j;
-        }
-        while (__any_sync(peers, cand != 0)) {
-            int32_t leaf_idx = -1;
-            while (cand != 0) {
-                const int32_t j = __ffsll((long long)cand) - 1;
-                cand &= cand - 1;
-                int32_t leaf;
-                if (entered(base + j, &leaf)) {
-                    leaf_idx = leaf;
-                    break;
-                }
-            }
-            __syncwarp(peers);
-
-            if (leaf_idx >= 0) {
-                float hit_t;
-                math::Vector3 leaf_normal;
-                if (traceRayIntoLeaf(leaf_idx, o, d, 0.f, t_max, &hit_t, &leaf_normal)) {
-                    t_max = hit_t;
-                    closest = unpackEntity(s_.leafEntities[leaf_idx]);
-                    closest_normal = leaf_normal;
-                }
-            }
-        }
-    }
-    if (closest == Entity::none()) return Entity::none();
-    *out_hit_t = t_max;
-    *out_hit_normal = closest_normal;
-    return closest;
+    float hit_t;
+    math::Vector3 hit_normal;
+    const int32_t leaf = mb2::physray::traceWorld(s_, s_.orderedBoxes, s_.numTraversal, __activemask(),
+                                                  o, d, t_max, &hit_t, &hit_normal);
+    if (leaf < 0) return Entity::none();
+    *out_hit_t = hit_t;
+    *out_hit_normal = hit_normal;
+    return unpackEntity(s_.leafEntities[leaf]);
 }
 
 }

@@ -57,6 +57,7 @@ EXPORTED_SYMBOLS = [
     "mb2_render_debug_hits",
     "mb2_render_debug_buffer",
     "mb2_render_free_views",
+    "mb2_trace_physics_rays",
     "mb2_peer_gather_create",
     "mb2_peer_gather_local_handle",
     "mb2_peer_gather_connect",
@@ -151,6 +152,15 @@ class _FreeViewC(ctypes.Structure):         # == mb2_free_view
 class _FreeViewOutputsC(ctypes.Structure):  # == mb2_free_view_outputs: device pointers or NULL
     _fields_ = [("rgb", ctypes.c_void_p), ("depth", ctypes.c_void_p),
                 ("segmentation", ctypes.c_void_p), ("normals", ctypes.c_void_p)]
+
+
+class _PhysicsRaysC(ctypes.Structure):      # == mb2_physics_rays: device pointers (max_t may be NULL)
+    _fields_ = [("world", ctypes.c_void_p), ("origin", ctypes.c_void_p), ("direction", ctypes.c_void_p),
+                ("max_t", ctypes.c_void_p)]
+
+
+class _PhysicsRayHitsC(ctypes.Structure):   # == mb2_physics_ray_hits: device pointers or NULL
+    _fields_ = [("entity", ctypes.c_void_p), ("t", ctypes.c_void_p), ("normal", ctypes.c_void_p)]
 
 
 class _SourceHullC(ctypes.Structure):
@@ -302,6 +312,9 @@ def load_library() -> ctypes.CDLL:
     lib.mb2_render_free_views.argtypes = [vp, ctypes.POINTER(_FreeViewC), ctypes.c_uint32, ctypes.c_uint32,
                                           ctypes.c_uint32, ctypes.c_uint32, ctypes.POINTER(_FreeViewOutputsC), vp]
     lib.mb2_render_free_views.restype = ctypes.c_int
+    lib.mb2_trace_physics_rays.argtypes = [vp, ctypes.POINTER(_PhysicsRaysC), ctypes.c_uint32,
+                                           ctypes.POINTER(_PhysicsRayHitsC), vp]
+    lib.mb2_trace_physics_rays.restype = ctypes.c_int
     lib.mb2_peer_gather_create.argtypes = [vp, ctypes.POINTER(ctypes.c_int64), ctypes.c_uint32,
                                            ctypes.POINTER(ctypes.c_uint64), ctypes.c_uint32, ctypes.c_uint32]
     lib.mb2_peer_gather_create.restype = vp
@@ -610,6 +623,56 @@ class MWCudaExecutor:
             else:
                 for t in out.values():
                     t.record_stream(target)
+        return out
+
+    def tracePhysicsRays(self, world, origin, direction, max_t=None, entity: bool = True, t: bool = True,
+                         normal: bool = True, stream=None):
+        """Trace a batch of rays against the worlds' collision geometry as the last step left it
+        (mb2_trace_physics_rays in include/madrona_b200.h): ray i gives what
+        BVH::traceRay(origin[i], direction[i], &t, &normal, max_t[i]) returns in world world[i].
+        world is int [n], origin and direction float [n, 3] (direction not normalised: t is in
+        its units), max_t float [n] or None for +inf; torch tensors or anything torch.as_tensor
+        takes, copied to this executor's GPU when they are elsewhere.  Returns a dict of new
+        tensors, those asked for: "entity" int32 [n, 2] {gen, id}, {-1, -1} on a miss; "t"
+        float32 [n], 0 on a miss; "normal" float32 [n, 3], world frame, 0 on a miss.
+        stream=None: synchronous on the executor's stream, like run(); a torch.cuda.Stream or
+        raw handle: enqueued there, the tensors recorded on it."""
+        import torch
+        dev = torch.device("cuda", self.gpu_id)
+
+        def dev_tensor(x, dtype, shape, name):
+            x = torch.as_tensor(x).to(device=dev, dtype=dtype).contiguous()
+            if tuple(x.shape) != shape:
+                raise ValueError(f"{name} has shape {tuple(x.shape)}, expected {shape}")
+            return x
+
+        world = torch.as_tensor(world)
+        n = int(world.shape[0]) if world.dim() > 0 else -1
+        if world.dim() != 1:
+            raise ValueError(f"world has shape {tuple(world.shape)}, expected [n]")
+        with torch.cuda.device(dev):
+            w = dev_tensor(world, torch.int32, (n,), "world")
+            o = dev_tensor(origin, torch.float32, (n, 3), "origin")
+            d = dev_tensor(direction, torch.float32, (n, 3), "direction")
+            m = None if max_t is None else dev_tensor(max_t, torch.float32, (n,), "max_t")
+            shapes = {"entity": ((n, 2), torch.int32), "t": ((n,), torch.float32), "normal": ((n, 3), torch.float32)}
+            wanted = {"entity": entity, "t": t, "normal": normal}
+            out = {k: torch.empty(shapes[k][0], dtype=shapes[k][1], device=dev) for k in shapes if wanted[k]}
+            s = self.stream if stream is None else int(getattr(stream, "cuda_stream", stream))
+            target = torch.cuda.ExternalStream(s, device=dev)
+            # the inputs and the new tensors are ordered on the current stream: the trace waits for it
+            target.wait_stream(torch.cuda.current_stream(dev))
+            rays = _PhysicsRaysC(w.data_ptr(), o.data_ptr(), d.data_ptr(), None if m is None else m.data_ptr())
+            hits = _PhysicsRayHitsC(*[out[k].data_ptr() if k in out else None for k in shapes])
+            if self._lib.mb2_trace_physics_rays(self._h, ctypes.byref(rays), n, ctypes.byref(hits),
+                                                ctypes.c_void_p(s)) != 0:
+                raise MadronaB200Error(_last_error(self._lib))
+            if stream is None:
+                target.synchronize()
+            else:
+                for x in [w, o, d, m] + list(out.values()):
+                    if x is not None:
+                        x.record_stream(target)
         return out
 
     def peerGather(self, slots, shapes, dtypes, world_size: int, rank: int):

@@ -198,6 +198,25 @@ struct FreeViewOutputs {
     void *normals;
 };
 
+// Rays for MWCudaExecutor::tracePhysicsRays (== mb2_physics_rays): device pointers, SoA and
+// contiguous -- world int32 [n], origin float [n][3], direction float [n][3] (not normalised),
+// max_t float [n] or nullptr for +inf.
+struct PhysicsRays {
+    const int32_t *world;
+    const float *origin;
+    const float *direction;
+    const float *maxT;
+};
+
+// Device pointers, or nullptr for an output not wanted: entity int32 [n][2] {gen, id}
+// (Entity::none() on a miss), t float [n] (0 on a miss), normal float [n][3] (world frame,
+// 0 on a miss).
+struct PhysicsRayHits {
+    int32_t *entity;
+    float *t;
+    float *normal;
+};
+
 // A device-memory snapshot of an executor's simulation state (include/madrona_b200.h),
 // made by MWCudaExecutor::snapshot().  save() / restore() are one kernel launch each on
 // `strm` (by default the executor's stream) and never synchronize the host; stepping after
@@ -396,6 +415,18 @@ public:
                                   image_size.height, (uint32_t)projection, &out, (void *)strm) != 0) {
             detail::fatal("renderFreeViews");
         }
+    }
+
+    // Not in the reference: trace n rays against the worlds' collision geometry as the last step
+    // left it, enqueued on `strm` (nullptr: the executor's stream) like runAsync
+    // (include/madrona_b200.h, mb2_trace_physics_rays).  Ray i gives what
+    // BVH::traceRay(origin[i], direction[i], &t, &normal, max_t[i]) returns in world world[i].
+    void tracePhysicsRays(::madrona_b200::PhysicsRays rays, uint32_t n, ::madrona_b200::PhysicsRayHits hits,
+                          cudaStream_t strm = nullptr)
+    {
+        const mb2_physics_rays r { rays.world, rays.origin, rays.direction, rays.maxT };
+        const mb2_physics_ray_hits h { hits.entity, hits.t, hits.normal };
+        if (mb2_trace_physics_rays(h_, &r, n, &h, (void *)strm) != 0) detail::fatal("tracePhysicsRays");
     }
 
     // Not in the reference: a snapshot of this executor's state (empty until its first save)

@@ -164,6 +164,31 @@ def _crowd_desc(name, two_archetypes=False):
     )
 
 
+def _rays_desc(name, spheres=False):
+    outputs = [Slot(0, "ray_origin", "float32", (64, 3)), Slot(1, "ray_dir", "float32", (64, 3)),
+               Slot(2, "ray_max_t", "float32", (64,)), Slot(3, "hit_entity", "int32", (64, 2)),
+               Slot(4, "hit_t", "float32", (64,)), Slot(5, "hit_normal", "float32", (64, 3)),
+               Slot(6, "body_count", "int32", (1,)),
+               Slot(7, "body_pos", "float32", (3,), dynamic=True),
+               Slot(8, "body_entity", "int32", (2,), dynamic=True)]
+    return SimDesc(
+        name=name,
+        sources=[os.path.join(_ROOT, "rays", "sim.cpp")],
+        num_exports=len(outputs),
+        num_taskgraphs=1,
+        inputs=[],
+        outputs=outputs,
+        pack_config=lambda cfg: struct.pack("<QIIII", int(cfg.get("obj_mgr_ptr", 0)), int(cfg["episode_len"]),
+                                            int(cfg["uniform_bodies"]), int(cfg["varied_bodies"]), 0),
+        pack_init=lambda w, cfg: struct.pack("<I", int(cfg.get("seed", 0)) + w),
+        oracle_extra=lambda cfg: [int(cfg.get("seed", 0)), int(cfg["episode_len"]), int(cfg["uniform_bodies"]),
+                                  int(cfg["varied_bodies"])],
+        defaults={"seed": 0, "episode_len": 12, "uniform_bodies": 0, "varied_bodies": 0},
+        objects=_hullpile_objects,
+        compile_flags=["-DRAYS_SPHERES=1"] if spheres else [],
+    )
+
+
 def _image_size(cfg, default_res):
     """Render config image size from the fixture config: keyword arguments for the
     render_assets builders.  `width` and `height` (both) give non-square images, else the
@@ -492,6 +517,12 @@ SIMS: Dict[str, SimDesc] = {
     # build variant with a second rigid-body archetype (every 4th dynamic body): its columns
     # as slots 5 - 8, and body_count also holds how many of the world's bodies it has
     "crowd2": _crowd_desc("crowd2", two_archetypes=True),
+    # traceRay probed in the simulator: 64 rays per world filled before physics from per-row RNGs,
+    # traced by the last node (tests/test_physics_rays.py); worlds of 8 to varied_bodies (0: 60)
+    # bodies, or uniform_bodies for all
+    "rays": _rays_desc("rays"),
+    # GPU only: the same fixture with spheres among the bodies
+    "rays_spheres": _rays_desc("rays_spheres", spheres=True),
     "gridworld": SimDesc(
         name="gridworld",
         sources=[os.path.join(_ROOT, "gridworld", "sim.cpp")],
