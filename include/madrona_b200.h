@@ -474,8 +474,20 @@ void mb2_navmesh_destroy(mb2_navmesh *navmesh);
  *              mb2_peer_gather_buffer(g, step & 1, i); release_async(g)
  * push / wait / release each advance their own step counter (kept on the
  * device), so they are CUDA-graph friendly.  bytes_per_slot[i] = bytes of ONE
- * rank's column (identical on all ranks, multiple of 4); buffer i of a parity
- * is [world_size][bytes_per_slot[i]], i.e. the world-major gathered column. */
+ * rank's column (identical on all ranks, any multiple of 4); buffer i of a parity
+ * is [world_size][bytes_per_slot[i]], i.e. the world-major gathered column.
+ *
+ * mb2_peer_gather_connect_local(gathers, n) connects the gathers of all ranks
+ * of ONE process on ONE GPU instead (cudaIpc cannot map memory into the
+ * process that exported it): gathers[r] is rank r's gather, n its world_size;
+ * each stores straight into the others' buffers.  It returns nonzero with
+ * mb2_last_error() set, and changes no gather, when a gather is null, n is not
+ * their world_size, a rank is missing or appears twice, their slot counts or
+ * bytes_per_slot differ, or they are on different GPUs.  The kernels of such
+ * ranks spin on each other's flags, so enqueue every rank's push, wait and
+ * release on ONE stream, in an order where each spin's condition already
+ * holds when it starts: per step k, every rank's run + push(k), then every
+ * rank's wait(k-1), read, release(k-1). */
 typedef struct mb2_peer_gather mb2_peer_gather;
 #define MB2_PEER_GATHER_HANDLE_BYTES 128
 mb2_peer_gather *mb2_peer_gather_create(mb2_executor *exec, const int64_t *slots,
@@ -483,6 +495,7 @@ mb2_peer_gather *mb2_peer_gather_create(mb2_executor *exec, const int64_t *slots
                                         uint32_t world_size, uint32_t rank);
 int mb2_peer_gather_local_handle(mb2_peer_gather *gather, void *handle_out);
 int mb2_peer_gather_connect(mb2_peer_gather *gather, const void *all_handles);
+int mb2_peer_gather_connect_local(mb2_peer_gather *const *gathers, uint32_t n);
 int mb2_peer_gather_push_async(mb2_peer_gather *gather, void *cuda_stream);
 int mb2_peer_gather_wait_async(mb2_peer_gather *gather, void *cuda_stream);
 int mb2_peer_gather_release_async(mb2_peer_gather *gather, void *cuda_stream);

@@ -61,6 +61,7 @@ EXPORTED_SYMBOLS = [
     "mb2_peer_gather_create",
     "mb2_peer_gather_local_handle",
     "mb2_peer_gather_connect",
+    "mb2_peer_gather_connect_local",
     "mb2_peer_gather_push_async",
     "mb2_peer_gather_wait_async",
     "mb2_peer_gather_release_async",
@@ -322,6 +323,8 @@ def load_library() -> ctypes.CDLL:
     lib.mb2_peer_gather_local_handle.restype = ctypes.c_int
     lib.mb2_peer_gather_connect.argtypes = [vp, ctypes.c_char_p]
     lib.mb2_peer_gather_connect.restype = ctypes.c_int
+    lib.mb2_peer_gather_connect_local.argtypes = [ctypes.POINTER(vp), ctypes.c_uint32]
+    lib.mb2_peer_gather_connect_local.restype = ctypes.c_int
     for name in ("push", "wait", "release"):
         fn = getattr(lib, f"mb2_peer_gather_{name}_async")
         fn.argtypes = [vp, vp]
@@ -1077,6 +1080,20 @@ class PeerGather:
         assert len(blob) == self.HANDLE_BYTES * self.world_size
         if self._lib.mb2_peer_gather_connect(self._h, blob) != 0:
             raise MadronaB200Error(_last_error(self._lib))
+
+    @staticmethod
+    def connect_local(gathers: Sequence["PeerGather"]) -> None:
+        """Connect the gathers of all ranks of one process on one GPU, gathers[r] being rank
+        r's, without cudaIpc (which cannot map memory into the process that exported it).
+        Their push / wait / release kernels spin on each other's flags, so they must all go
+        on one stream, each step every rank's run and push(k), then every rank's
+        wait(k - 1), read and release(k - 1) (include/madrona_b200.h).  A closed gather
+        counts as a null one."""
+        lib = load_library()
+        gathers = list(gathers)
+        handles = (ctypes.c_void_p * len(gathers))(*[g._h for g in gathers])
+        if lib.mb2_peer_gather_connect_local(handles, len(gathers)) != 0:
+            raise MadronaB200Error(_last_error(lib))
 
     def _call(self, name, stream):
         s = getattr(stream, "cuda_stream", stream)
