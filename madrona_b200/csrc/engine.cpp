@@ -11,6 +11,7 @@
 #include "engine.hpp"
 #include "physics_host.hpp"
 #include "physics_state.h"
+#include "render_state.h"
 
 #include <cstdio>
 #include <cstdlib>
@@ -83,6 +84,8 @@ static std::string describeErrors(uint32_t flags, uint32_t archetype)
     if (flags & ErrRenderCapacity) s += "render instance list overflow ";
     if (flags & ErrRenderTLASDepth) s += "render TLAS too deep for the ray caster's traversal stack (a world's "
         "renderables are too tightly clustered) ";
+    if (flags & ErrRenderLights) s += "more than " + std::to_string(kMaxLightsPerWorld) + " render lights in a "
+        "world (the first " + std::to_string(kMaxLightsPerWorld) + " were drawn) ";
     return s;
 }
 

@@ -317,8 +317,13 @@ renderGatherLightsKernel(EngineState *Sp)
         const i32 first = t.worldOffsets[w];
         const i32 count = t.worldCounts[w];
         i32 kept = 0;
-        for (i32 r = first; r < first + count && kept < kMaxLightsPerWorld; r++) {
+        for (i32 r = first; r < first + count; r++) {
             if (((const i32 *)t.columns[1])[r] != w) continue;
+            // a live light past the cap is reported (ErrRenderLights) and not drawn
+            if (kept == kMaxLightsPerWorld) {
+                atomicOr(&S.errorFlags, (u32)ErrRenderLights);
+                break;
+            }
             const LightDescComp d = ((const LightDescComp *)t.columns[R.lightCol])[r];
             RenderLight l;
             l.directional = d.type ? 1u : 0u;

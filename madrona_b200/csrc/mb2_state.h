@@ -241,6 +241,7 @@ enum ErrorFlags : u32 {
     ErrTooManyNodeDatas = 1u << 10,    // more custom node datas than kMaxNodeDatas
     ErrNavmeshPolygon = 1u << 11,      // Navmesh::initFromPolygons got a polygon of fewer than 3 vertices
     ErrPhysicsRayWorld = 1u << 12,     // mb2_trace_physics_rays got a ray of a world outside [0, numWorlds)
+    ErrRenderLights = 1u << 13,        // a world has more live lights than kMaxLightsPerWorld
 };
 
 }

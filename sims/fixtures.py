@@ -422,6 +422,29 @@ SIMS: Dict[str, SimDesc] = {
         render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_render_config(
             rgbd=bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)), **_render_options(cfg, 40)),
     ),
+    # GPU only: the gallery built with -DGALLERY_LIGHTS=1 (tests/test_render_lights.py): lamps[w]
+    # lamps in world w, moved and retyped every step; every lamp_period steps (0: never) a
+    # respawn leaves lamps_after[w] (then lamps[w], ...) of them.  Slots 13 - 19 / 20 - 26: the
+    # Lamp / Beacon carrier rows' position, direction, type, shadow flag, cutoff, light entity
+    # and world
+    "gallery_lit": SimDesc(
+        name="gallery_lit",
+        sources=[os.path.join(_ROOT, "gallery", "sim.cpp")],
+        num_exports=27,
+        num_taskgraphs=1,
+        inputs=[],
+        outputs=[],
+        pack_config=lambda cfg: struct.pack("<III", int(cfg["num_props"]), 5, int(cfg["lamp_period"])),
+        pack_init=lambda w, cfg: struct.pack("<III", int(cfg.get("seed", 0)) + w, int(cfg["lamps"][w]),
+                                             int(cfg["lamps_after"][w] if cfg.get("lamps_after") else
+                                                 cfg["lamps"][w])),
+        oracle_extra=lambda cfg: [],
+        defaults={"num_props": 100, "lamps": [2], "lamps_after": None, "lamp_period": 0, "seed": 0,
+                  "resolution": 40, "rgbd": True},
+        compile_flags=["-DGALLERY_LIGHTS=1", "-DGALLERY_ENTITY_EXPORTS=1", "-DGALLERY_NORMAL_EXPORTS=1"],
+        render=lambda cfg: __import__("sims.render_assets", fromlist=["x"]).make_gallery_render_config(
+            rgbd=bool(cfg.get("rgbd", True)), gpu_id=int(cfg.get("_gpu_id", 0)), **_render_options(cfg, 40)),
+    ),
     # GPU only: the gallery sim with uvs and textured materials (tests/test_render_textures.py);
     # same sources and flags, so it shares the gallery's simulator module
     "gallery_textured": SimDesc(

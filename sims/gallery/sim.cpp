@@ -14,7 +14,16 @@ void Sim::registerTypes(ECSRegistry &registry, const Config &)
     registry.registerComponent<Spin>();
     registry.registerArchetype<Prop>();
     registry.registerArchetype<Viewer>(ComponentMetadataSelector<> {}, ArchetypeFlags::None, kNumViews);
+#if defined(GALLERY_LIGHTS)
+    registry.registerComponent<LampMotion>();
+    registry.registerComponent<BeaconTag>();
+    registry.registerSingleton<LampClock>();
+    // a respawn's new rows coexist with the destroyed ones until the compaction
+    registry.registerArchetype<Lamp>(ComponentMetadataSelector<> {}, ArchetypeFlags::None, 2 * kNumLights);
+    registry.registerArchetype<Beacon>(ComponentMetadataSelector<> {}, ArchetypeFlags::None, 2 * kNumLights + 1);
+#else
     registry.registerArchetype<Lamp>(ComponentMetadataSelector<> {}, ArchetypeFlags::None, kNumLights);
+#endif
 
     registry.exportColumn<Prop, Position>((uint32_t)ExportID::PropPos);
     registry.exportColumn<Prop, Rotation>((uint32_t)ExportID::PropRot);
@@ -33,6 +42,22 @@ void Sim::registerTypes(ECSRegistry &registry, const Config &)
     registry.exportColumn<RaycastOutputArchetype, NormalOutputBuffer>((uint32_t)ExportID::Normals);
 #endif
 #endif
+#if defined(GALLERY_LIGHTS)
+    registry.exportColumn<Lamp, Position>((uint32_t)ExportID::LampPos);
+    registry.exportColumn<Lamp, LightDescDirection>((uint32_t)ExportID::LampDir);
+    registry.exportColumn<Lamp, LightDescType>((uint32_t)ExportID::LampType);
+    registry.exportColumn<Lamp, LightDescShadow>((uint32_t)ExportID::LampShadow);
+    registry.exportColumn<Lamp, LightDescCutoffAngle>((uint32_t)ExportID::LampCutoff);
+    registry.exportColumn<Lamp, LightCarrier>((uint32_t)ExportID::LampLight);
+    registry.exportColumn<Lamp, WorldID>((uint32_t)ExportID::LampWorld);
+    registry.exportColumn<Beacon, Position>((uint32_t)ExportID::BeaconPos);
+    registry.exportColumn<Beacon, LightDescDirection>((uint32_t)ExportID::BeaconDir);
+    registry.exportColumn<Beacon, LightDescType>((uint32_t)ExportID::BeaconType);
+    registry.exportColumn<Beacon, LightDescShadow>((uint32_t)ExportID::BeaconShadow);
+    registry.exportColumn<Beacon, LightDescCutoffAngle>((uint32_t)ExportID::BeaconCutoff);
+    registry.exportColumn<Beacon, LightCarrier>((uint32_t)ExportID::BeaconLight);
+    registry.exportColumn<Beacon, WorldID>((uint32_t)ExportID::BeaconWorld);
+#endif
 }
 
 // props turn about z by a fixed small step (cos, sin of 0.02 rad as literals) and bob
@@ -46,11 +71,113 @@ inline void spinSystem(Engine &, Position &pos, Rotation &rot, Spin &spin)
     pos.z += 0.01f * spin.phase;
 }
 
+#if defined(GALLERY_LIGHTS)
+// a lamp of a random kind (directional, spotlight with a 0.3 - 1.3 rad cone, or point light:
+// a spotlight with cutoff -1), shadow flag, intensity and active flag, anchored among the props
+// (whose centres lie 0.6 - 3.1 above the floor) or above them, pointing down at a tilt
+template <typename ArchetypeT>
+static Entity makeLampOf(Engine &ctx, Sim &sim)
+{
+    Entity e = ctx.makeEntity<ArchetypeT>();
+    if (e.id < 0) return e;
+    RNG &rng = sim.rng;
+    const int32_t kind = rng.sampleI32(0, 3);
+    LampMotion m;
+    m.anchor = Vector3 { (rng.sampleUniform() - 0.5f) * 20.f, (rng.sampleUniform() - 0.5f) * 20.f,
+                         0.8f + 5.f * rng.sampleUniform() };
+    m.phase = 6.2831853f * rng.sampleUniform();
+    m.heading = 6.2831853f * rng.sampleUniform();
+    m.tilt = 0.15f + 0.75f * rng.sampleUniform();
+    m.index = sim.lampsMade++;
+    ctx.get<LampMotion>(e) = m;
+    ctx.get<Position>(e) = m.anchor;
+    ctx.get<LightDescDirection>(e) =
+        LightDescDirection(Vector3 { m.tilt * cosf(m.heading), m.tilt * sinf(m.heading), -1.f }.normalize());
+    ctx.get<LightDescType>(e).type = kind == 0 ? LightDesc::Directional : LightDesc::Spotlight;
+    ctx.get<LightDescShadow>(e).castShadow = rng.sampleBool();
+    const float cone = 0.3f + rng.sampleUniform();
+    ctx.get<LightDescCutoffAngle>(e).cutoff = kind == 2 ? -1.f : cone;
+    ctx.get<LightDescIntensity>(e).intensity = 0.25f + 1.75f * rng.sampleUniform();
+    ctx.get<LightDescActive>(e).active = rng.sampleUniform() < 0.75f;
+    RenderingSystem::makeEntityLightCarrier(ctx, e);
+    return e;
+}
+
+// every third lamp a world makes is a Beacon
+static Entity makeLamp(Engine &ctx, Sim &sim)
+{
+    if (sim.lampsMade % 3 == 1) {
+        const uint32_t index = sim.lampsMade;
+        Entity e = makeLampOf<Beacon>(ctx, sim);
+        if (e.id >= 0) ctx.get<BeaconTag>(e).index = index;
+        return e;
+    }
+    return makeLampOf<Lamp>(ctx, sim);
+}
+
+static void destroyLamp(Engine &ctx, Entity lamp)
+{
+    const Entity light = ctx.get<LightCarrier>(lamp).light;
+    if (light.id >= 0) ctx.destroyEntity(light);
+    ctx.destroyEntity(lamp);
+}
+
+inline void lampClockSystem(Engine &, LampClock &c)
+{
+    c.t += 1;
+}
+
+// lamps of both carrier archetypes: circle the anchor, turn, flip shadow flag and type now and then
+inline void lampSystem(Engine &ctx, Position &pos, LightDescDirection &dir, LightDescType &type,
+                       LightDescShadow &shadow, LampMotion &m)
+{
+    const uint32_t t = ctx.singleton<LampClock>().t + m.index;
+    m.phase += 0.35f;
+    m.heading += 0.25f;
+    pos = m.anchor + Vector3 { 1.2f * cosf(m.phase), 1.2f * sinf(m.phase), 0.4f * sinf(0.7f * m.phase) };
+    dir = LightDescDirection(Vector3 { m.tilt * cosf(m.heading), m.tilt * sinf(m.heading), -1.f }.normalize());
+    if (t % 3 == 0) shadow.castShadow = !shadow.castShadow;
+    if (t % 4 == 0) {
+        type.type = type.type == LightDesc::Directional ? LightDesc::Spotlight : LightDesc::Directional;
+    }
+}
+
+// one thread per world: every lampPeriod steps, destroy every other lamp (with its light
+// entity) and any past the new count, then make lamps up to it
+inline void lampRespawnSystem(Engine &ctx, LampClock &c)
+{
+    Sim &sim = ctx.data();
+    if (sim.lampPeriod == 0 || c.t % sim.lampPeriod != 0) return;
+    sim.respawns++;
+    const uint32_t target = (sim.respawns & 1) ? sim.lampsAfter : sim.numLampsInit;
+    uint32_t kept = 0;
+    for (uint32_t i = 0; i < sim.numLamps; i++) {
+        if (i % 2 == 0 || kept >= target) {
+            destroyLamp(ctx, sim.lamps[i]);
+        } else {
+            sim.lamps[kept++] = sim.lamps[i];
+        }
+    }
+    while (kept < target) sim.lamps[kept++] = makeLamp(ctx, sim);
+    sim.numLamps = kept;
+}
+#endif
+
 void Sim::setupTasks(TaskGraphManager &mgr, const Config &)
 {
     TaskGraphBuilder &builder = mgr.init(TaskGraphID::Step);
     auto spin = builder.addToGraph<ParallelForNode<Engine, spinSystem, Position, Rotation, Spin>>({});
+#if defined(GALLERY_LIGHTS)
+    auto clock = builder.addToGraph<ParallelForNode<Engine, lampClockSystem, LampClock>>({spin});
+    auto move = builder.addToGraph<ParallelForNode<Engine, lampSystem, Position, LightDescDirection, LightDescType,
+                                                   LightDescShadow, LampMotion>>({clock});
+    auto respawn = builder.addToGraph<ParallelForNode<Engine, lampRespawnSystem, LampClock>>({move});
+    auto lamps = builder.addToGraph<CompactArchetypeNode<Lamp>>({respawn});
+    auto beacons = builder.addToGraph<CompactArchetypeNode<Beacon>>({lamps});
+    RenderingSystem::setupTasks(builder, {beacons});
+#else
     RenderingSystem::setupTasks(builder, {spin});
+#endif
 }
 
 Sim::Sim(Engine &ctx, const Config &cfg, const WorldInit &init)
@@ -120,6 +247,29 @@ Sim::Sim(Engine &ctx, const Config &cfg, const WorldInit &init)
         RenderingSystem::attachEntityToView(ctx, e, 70.f, 0.001f, Vector3 { 0.f, 0.f, 0.25f });
     }
 
+#if defined(GALLERY_LIGHTS)
+    lampPeriod = cfg.lampPeriod;
+    numLampsInit = init.numLamps < (uint32_t)kNumLights ? init.numLamps : (uint32_t)kNumLights;
+    lampsAfter = init.lampsAfter < (uint32_t)kNumLights ? init.lampsAfter : (uint32_t)kNumLights;
+    respawns = 0;
+    lampsMade = 0;
+    ctx.singleton<LampClock>().t = 0;
+    for (numLamps = 0; numLamps < numLampsInit; numLamps++) lamps[numLamps] = makeLamp(ctx, *this);
+    // a carrier that carries no light: the light refresh must pass it by
+    {
+        Entity e = ctx.makeEntity<Beacon>();
+        ctx.get<Position>(e) = Vector3 { 0.f, 0.f, 5.f };
+        ctx.get<LightDescDirection>(e) = LightDescDirection(Vector3 { 0.f, 0.f, -1.f });
+        ctx.get<LightDescType>(e).type = LightDesc::Directional;
+        ctx.get<LightDescShadow>(e).castShadow = false;
+        ctx.get<LightDescCutoffAngle>(e).cutoff = 0.5f;
+        ctx.get<LightDescIntensity>(e).intensity = 1.f;
+        ctx.get<LightDescActive>(e).active = true;
+        ctx.get<LampMotion>(e) = LampMotion { Vector3 { 0.f, 0.f, 5.f }, 0.f, 0.f, 0.5f, 0u };
+        ctx.get<BeaconTag>(e).index = 0xFFFFFFFFu;
+        ctx.get<LightCarrier>(e).light = Entity::none();
+    }
+#else
     for (int32_t l = 0; l < kNumLights; l++) {
         Entity e = ctx.makeEntity<Lamp>();
         ctx.get<Position>(e) = Vector3 { 0.f, 0.f, 9.f };
@@ -132,6 +282,7 @@ Sim::Sim(Engine &ctx, const Config &cfg, const WorldInit &init)
         ctx.get<LightDescActive>(e).active = true;
         RenderingSystem::makeEntityLightCarrier(ctx, e);
     }
+#endif
 }
 
 }
